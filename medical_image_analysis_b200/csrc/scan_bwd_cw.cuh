@@ -82,7 +82,7 @@ __device__ __forceinline__ void cw_bwd_block(const int qlo_in, const int qhi_in,
                                              float2 &dA2, float2 &dD2, float2 &db2) {
     constexpr int es = (int)sizeof(T), eo = (int)sizeof(TO);
     const int qlo = kFull ? 0 : qlo_in, qhi = kFull ? 4 : qhi_in;
-    const float2 kL2E = splat2(kLog2e), kOne = splat2(1.f);
+    const float2 kL2E = splat2(kLog2e);
     const int i16 = lane & 15;
     const bool mine = kFull || (i16 >= 4 * qlo && i16 < 4 * qhi);       // this lane's butterfly slot is a token of the block
     CwRegs R;
@@ -125,9 +125,7 @@ __device__ __forceinline__ void cw_bwd_block(const int qlo_in, const int qhi_in,
                 const int k = 2 * q0 + p;
                 float2 m = fma2(dd[p], kL2E, bl2);                      // (delta + bias) log2e
                 if (kSoftplus) {
-                    const float2 e = make_float2(ex2f(fminf(m.x, 120.f)), ex2f(fminf(m.y, 120.f)));
-                    const float2 s = add2(e, kOne);
-                    m = make_float2(fmaxf(lg2f(s.x), m.x), fmaxf(lg2f(s.y), m.y));   // softplus log2e
+                    m = softplus_l2(m);   // softplus log2e
                 }
                 const float2 av = ex2_2(mul2(m, A2));
                 const float2 bv = mul2(mul2(m, uu[p]), Bv[p]);
@@ -171,7 +169,7 @@ __device__ __forceinline__ void cw_bwd_block(const int qlo_in, const int qhi_in,
                 const float2 dBv = mul2(gg, mul2(R.m[k], uu[p]));
                 v[2 * k] = dBv.x; v[2 * k + 1] = dBv.y;
                 float2 sg = kL2E;                                       // d m / d (delta + bias) = sigmoid log2e = (1 - 2^-m) log2e
-                if (kSoftplus) sg = fma2(ex2_2(make_float2(-R.m[k].x, -R.m[k].y)), make_float2(-kLog2e, -kLog2e), kL2E);
+                if (kSoftplus) sg = sigmoid_of_softplus_l2(R.m[k], kLog2e);
                 const float2 qv = fma2(R.hp[k], Aln2, mul2(uu[p], Bv[p]));   // ln2 d h_t / d m_t
                 du[p] = fma2(gg, mul2(R.m[k], Bv[p]), mul2(dy[p], D2));
                 dd[p] = mul2(gg, mul2(qv, sg));

@@ -55,7 +55,7 @@ __global__ void __launch_bounds__(kThreads, 1) ss_bwd_fast_kernel(const __grid_c
     const uint32_t dpitch = a.flat_delta ? (uint32_t)(L * es) : (uint32_t)a.row_pitch, dstep = a.flat_delta ? 0u : dstepB;
     const uint32_t opitch = a.flat_dout ? (uint32_t)(L * eso) : (uint32_t)a.rowo_pitch, ostep = a.flat_dout ? 0u : ostepB;
     const size_t du_step = (size_t)a.du_ds * es, dd_step = (size_t)a.dd_ds * es;
-    const float2 kL2E = splat2(kLog2e), kOne = splat2(1.f), kLN2 = splat2(kLn2);
+    const float2 kL2E = splat2(kLog2e), kLN2 = splat2(kLn2);
     int kr = 0, kg = 0;
     for (int seg = blockIdx.x; seg < a.n_seg; seg += gridDim.x) {
         const SegCoord sc = decode_seg(a, seg);
@@ -119,11 +119,10 @@ __global__ void __launch_bounds__(kThreads, 1) ss_bwd_fast_kernel(const __grid_c
                     for (int k = 0; k < 4; ++k) {
                         float2 m = fma2(m2[k], kL2E, bl);       // (delta + bias) * log2e
                         if (kSoftplus) {
-                            const float2 e = make_float2(ex2f(fminf(m.x, 120.f)), ex2f(fminf(m.y, 120.f)));
-                            const float2 s = add2(e, kOne);
+                            float2 e;
+                            m = softplus_l2(m, e);                                              // softplus * log2e
                             const float2 sl = fma2(e, kLN2, kLN2);                              // (1 + e) ln2
                             sg2[k] = mul2(e, make_float2(rcpf(sl.x), rcpf(sl.y)));              // sigmoid * log2e
-                            m = make_float2(fmaxf(lg2f(s.x), m.x), fmaxf(lg2f(s.y), m.y));      // softplus * log2e
                         } else {
                             sg2[k] = kL2E;
                         }

@@ -57,7 +57,7 @@ struct BlkRegs {
 template <typename T, bool kSoftplus>
 __device__ __forceinline__ void recompute_quad(BlkRegs &R, int q, const char *pu, const char *pd, const float *Bq, float &h,
                                                const float2 bl2, const float2 A2, const float2 Aln2) {
-    const float2 kL2E = splat2(kLog2e), kOne = splat2(1.f), kLN2 = splat2(kLn2);
+    const float2 kL2E = splat2(kLog2e), kLN2 = splat2(kLn2);
     float2 dd[2], uu[2], Bv[2];
     Quad<T>::ld(pd, dd);
     Quad<T>::ld(pu, uu);
@@ -68,11 +68,10 @@ __device__ __forceinline__ void recompute_quad(BlkRegs &R, int q, const char *pu
         float2 m = fma2(dd[p], kL2E, bl2);                      // (delta + bias) log2e
         float2 sg = kL2E;
         if (kSoftplus) {
-            const float2 e = make_float2(ex2f(fminf(m.x, 120.f)), ex2f(fminf(m.y, 120.f)));
-            const float2 s = add2(e, kOne);
+            float2 e;
+            m = softplus_l2(m, e);
             const float2 sl = fma2(e, kLN2, kLN2);              // (1 + e) ln2
             sg = mul2(e, make_float2(rcpf(sl.x), rcpf(sl.y)));  // sigmoid log2e
-            m = make_float2(fmaxf(lg2f(s.x), m.x), fmaxf(lg2f(s.y), m.y));
         }
         const float2 av = ex2_2(mul2(m, A2));
         const float2 mu = mul2(m, uu[p]);
@@ -156,7 +155,7 @@ template <typename T, typename TO, bool kSoftplus, bool kSecond, bool kFull>
 __device__ __forceinline__ void phase1_block(const int t0, const int nq, const char *pu, const char *pd, const char *po, const float *Bf,
                                              const float *Cf, const float2 bl2, const float2 A2, float &h, float2 &msum, float &P, float &Gs) {
     constexpr int es = (int)sizeof(T), eo = (int)sizeof(TO);
-    const float2 kL2E = splat2(kLog2e), kOne = splat2(1.f);
+    const float2 kL2E = splat2(kLog2e);
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
         if (kFull || q < nq) {
@@ -173,9 +172,7 @@ __device__ __forceinline__ void phase1_block(const int t0, const int nq, const c
             for (int p = 0; p < 2; ++p) {
                 float2 m = fma2(dd[p], kL2E, bl2);
                 if (kSoftplus) {
-                    const float2 e = make_float2(ex2f(fminf(m.x, 120.f)), ex2f(fminf(m.y, 120.f)));
-                    const float2 s = add2(e, kOne);
-                    m = make_float2(fmaxf(lg2f(s.x), m.x), fmaxf(lg2f(s.y), m.y));
+                    m = softplus_l2(m);
                 }
                 const float2 av = ex2_2(mul2(m, A2));
                 const float2 bv = mul2(mul2(m, uu[p]), Bv[p]);

@@ -215,7 +215,7 @@ __global__ void __launch_bounds__(32 * kRnWarps, 3) ss_bwd_rowsn_kernel(const __
                     const int idx = (qi * 4 + r) * L + t;
                     uv = raw_at<T>(raw_u, idx);
                     m = fmaf(raw_at<T>(raw_d, idx), kLog2e, bias_l2);
-                    if (kSoftplus) m = fmaxf(lg2f(1.f + ex2f(fminf(m, 120.f))), m);
+                    if (kSoftplus) m = softplus_l2(m);
                     dy = raw_at<TO>(raw_o, idx);
                     if (kHasZ) {
                         // out_z = y silu(z): dy = dout silu(z); dz = dout y sigmoid(z) (1 + z (1 - sigmoid(z)))  (y = saved out)
@@ -374,7 +374,7 @@ __global__ void __launch_bounds__(32 * kRnWarps, 3) ss_bwd_rowsn_kernel(const __
                     const int t = t0 + sp;
                     const float mt = mrow[t], ut = urow[t], dyt = yrow[t];
                     float ddl = fmaf(ut, s[0], s[1]);
-                    if (kSoftplus) ddl *= 1.f - ex2f(-mt);                     // sigmoid(x) = 1 - exp(-softplus(x)) = 1 - 2^(-m)
+                    if (kSoftplus) ddl *= sigmoid_of_softplus_l2(mt, 1.f);      // sigmoid(x) = 1 - exp(-softplus(x)) = 1 - 2^(-m)
                     const float duv = fmaf(dyt, Dv, mt * kLn2 * s[0]);
                     dbl += ddl;
                     dDl = fmaf(dyt, ut, dDl);

@@ -97,16 +97,50 @@ __device__ __forceinline__ float ex2f(float x) { float y; asm("ex2.approx.ftz.f3
 __device__ __forceinline__ float lg2f(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcpf(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
+// Softplus in the log2 domain, the form every scan kernel uses: m(x) = log2(1 + 2^x) = softplus(x ln2) log2e, with
+// e = 2^min(x, 120) handed back (the clamp keeps 2^. finite, the max restores x where the clamp bit; for x log2e > 20 the
+// log term equals x to fp32 precision, which is the reference's `x <= 20 ? log1p(exp(x)) : x`, fwd_kernel_oflex.cuh:126).
+// m enters du, ddelta and y as a FACTOR (dl u B), so it is its RELATIVE error that counts, and trained models sit at
+// delta + bias = x ln2 in about [-8, -1] where m ~ e is small: lg2(1 + e) alone is good to an ulp of 1.0 (the sum drops
+// the low bits of e, and lg2.approx is specified to 2^-22 ABSOLUTE on (0.5, 2)), i.e. to 6e-8 / e relative - 6e-5 at -7.  Below
+// e = 1/4 the value is e P(e) instead, P = the degree-4 interpolant of log2(1 + e) / e on [0, 1/4] (3e-7 relative in fp32,
+// ex2.approx's 2 ulp on e included in neither); above, lg2(1 + e) >= 0.32 and the absolute bound is 1e-6 relative.
+__device__ __forceinline__ float softplus_l2(float x, float &e) {
+    e = ex2f(fminf(x, 120.f));
+    float p = fmaf(e, 1.784831882e-01f, -3.390570283e-01f);
+    p = fmaf(p, e, 4.790599346e-01f);
+    p = fmaf(p, e, -7.212913036e-01f);
+    p = fmaf(p, e, 1.442694783e+00f);
+    const float big = fmaxf(lg2f(1.f + e), x);
+    return e < 0.25f ? e * p : big;
+}
+__device__ __forceinline__ float softplus_l2(float x) { float e; return softplus_l2(x, e); }
+__device__ __forceinline__ float2 softplus_l2(float2 x) { return make_float2(softplus_l2(x.x), softplus_l2(x.y)); }
+__device__ __forceinline__ float2 softplus_l2(float2 x, float2 &e) { return make_float2(softplus_l2(x.x, e.x), softplus_l2(x.y, e.y)); }
+
+// scale * sigmoid(x ln2) from m = softplus_l2(x), for kernels that keep m and not e: sigmoid = e / (1 + e) = 1 - 2^-m
+// (the x > 20 branch included: there it is 1 to fp32 precision).  The difference cancels for small m (relative error
+// 3e-7 / m), so below m = log2(5/4) - the same switch point as softplus_l2 - it is m Q(m), Q = the cubic interpolant of
+// (1 - 2^-m) / m (3e-7 relative in fp32).
+__device__ __forceinline__ float sigmoid_of_softplus_l2(float m, float scale) {
+    float q = fmaf(m, -8.801935241e-03f, 5.534247309e-02f);
+    q = fmaf(q, m, -2.402161658e-01f);
+    q = fmaf(q, m, 6.931470633e-01f);
+    const float big = fmaf(ex2f(-m), -scale, scale);
+    return m < 0.3219281f ? (m * scale) * q : big;
+}
+__device__ __forceinline__ float2 sigmoid_of_softplus_l2(float2 m, float scale) {
+    return make_float2(sigmoid_of_softplus_l2(m.x, scale), sigmoid_of_softplus_l2(m.y, scale));
+}
+
 // softplus(x) = log1p(exp(x)) for x <= 20, x above (fwd_kernel_oflex.cuh:126), and optionally its derivative
-// sigmoid(x) (bwd_kernel_oflex.cuh:252-257).  Evaluated as max(lg2(1 + 2^min(x log2e, 120)) ln2, x): for 20 < x the
-// log1p term equals x to fp32 precision, the clamp keeps 2^. finite, the max restores x where the clamp bit.
-// Absolute error <= 1 ulp of 1.0 (6e-8), which is what enters exp(dl A) and dl u B.
+// sigmoid(x) = e / (1 + e) (bwd_kernel_oflex.cuh:252-257), in natural units for the generic warp-scan kernels.
 template <bool kWithSigmoid>
 __device__ __forceinline__ float softplus_f(float x, float &sig) {
-    const float e = ex2f(fminf(x * kLog2e, 120.f));
-    const float s = 1.f + e;
-    if (kWithSigmoid) sig = e * rcpf(s);
-    return fmaxf(lg2f(s) * kLn2, x);
+    float e;
+    const float m = softplus_l2(x * kLog2e, e);
+    if (kWithSigmoid) sig = e * rcpf(1.f + e);
+    return fmaxf(m * kLn2, x);
 }
 
 // ------------------------------------------------------------------------------------------------

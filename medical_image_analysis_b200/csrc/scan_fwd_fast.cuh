@@ -49,7 +49,7 @@ __global__ void __launch_bounds__(kThreadsFwd, 1) ss_fwd_fast_kernel(const __gri
     const uint32_t dpitch = a.flat_delta ? (uint32_t)(L * es) : (uint32_t)a.row_pitch, dstep = a.flat_delta ? 0u : dstepB;
     const size_t out_step = (size_t)a.out_ds * eo;
     const size_t xstride = (size_t)a.n_chunks;
-    const float2 kL2E = splat2(kLog2e), kOne = splat2(1.f);
+    const float2 kL2E = splat2(kLog2e);
     int kr = 0, kg = 0;
     for (int seg = blockIdx.x; seg < a.n_seg; seg += gridDim.x) {
         const SegCoord sc = decode_seg(a, seg);
@@ -98,9 +98,7 @@ __global__ void __launch_bounds__(kThreadsFwd, 1) ss_fwd_fast_kernel(const __gri
                     for (int k = 0; k < 4; ++k) {
                         float2 m = fma2(d2[k], kL2E, bl);       // (delta + bias) * log2e
                         if (kSoftplus) {
-                            const float2 e = make_float2(ex2f(fminf(m.x, 120.f)), ex2f(fminf(m.y, 120.f)));
-                            const float2 s = add2(e, kOne);
-                            m = make_float2(fmaxf(lg2f(s.x), m.x), fmaxf(lg2f(s.y), m.y));   // softplus * log2e
+                            m = softplus_l2(m);   // softplus * log2e
                         }
                         y2[k] = mul2(u2[k], splat2(Dv));
                         const float2 arg = mul2(m, splat2(Araw));

@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(32 * kRowsNWarps) ss_fwd_rowsn_kernel(const __
     const float *Ap = reinterpret_cast<const float *>(a.A);
     const float *Dp = reinterpret_cast<const float *>(a.D);
     const float *biasp = reinterpret_cast<const float *>(a.delta_bias);
-    const float2 kL2E = splat2(kLog2e), kOne = splat2(1.f);
+    const float2 kL2E = splat2(kLog2e);
     char *pu = tu + (size_t)lane * L * es;
     const char *pd = td + (size_t)lane * L * es;
     char *pz = tz + (size_t)lane * L * es;
@@ -194,9 +194,7 @@ __global__ void __launch_bounds__(32 * kRowsNWarps) ss_fwd_rowsn_kernel(const __
                 for (int qq = 0; qq < 2; ++qq) {
                     float2 m = fma2(dd[qq], kL2E, bl2);         // (delta + bias) * log2e
                     if (kSoftplus) {
-                        const float2 e = make_float2(ex2f(fminf(m.x, 120.f)), ex2f(fminf(m.y, 120.f)));
-                        const float2 sp = add2(e, kOne);
-                        m = make_float2(fmaxf(lg2f(sp.x), m.x), fmaxf(lg2f(sp.y), m.y));   // softplus * log2e
+                        m = softplus_l2(m);   // softplus * log2e
                     }
                     mm[2 * qq] = m.x; mm[2 * qq + 1] = m.y;
                 }
@@ -226,7 +224,7 @@ __global__ void __launch_bounds__(32 * kRowsNWarps) ss_fwd_rowsn_kernel(const __
                 const float dl = Cvt<T>::to_f(*reinterpret_cast<const raw *>(pd + t * es));
                 const float uval = Cvt<T>::to_f(*reinterpret_cast<const raw *>(pu + t * es));
                 float m = fmaf(dl, kLog2e, bl2.x);
-                if (kSoftplus) m = fmaxf(lg2f(1.f + ex2f(fminf(m, 120.f))), m);
+                if (kSoftplus) m = softplus_l2(m);
                 const float yv = token(m, uval, t);
                 if (kOutF32) *reinterpret_cast<float *>(orow + (size_t)t * 4) = yv;
                 else *reinterpret_cast<raw *>(pu + t * es) = Cvt<T>::from_f(yv);

@@ -58,7 +58,7 @@ __global__ void __launch_bounds__(32, 16) ss_fwd_stream_kernel(const __grid_cons
     const float *Ap = reinterpret_cast<const float *>(a.A);
     const float *Dp = reinterpret_cast<const float *>(a.D);
     const float *biasp = reinterpret_cast<const float *>(a.delta_bias);
-    const float2 kL2E = splat2(kLog2e), kOne = splat2(1.f);
+    const float2 kL2E = splat2(kLog2e);
     using raw = typename Cvt<T>::raw;
 
     for (int item = blockIdx.x; item < a.n_items; item += gridDim.x) {
@@ -134,9 +134,7 @@ __global__ void __launch_bounds__(32, 16) ss_fwd_stream_kernel(const __grid_cons
                 for (int p = 0; p < 2; ++p) {
                     float2 m = fma2(dd[p], kL2E, bl2);       // (delta + bias) * log2e
                     if (kSoftplus) {
-                        const float2 e = make_float2(ex2f(fminf(m.x, 120.f)), ex2f(fminf(m.y, 120.f)));
-                        const float2 sp = add2(e, kOne);
-                        m = make_float2(fmaxf(lg2f(sp.x), m.x), fmaxf(lg2f(sp.y), m.y));   // softplus * log2e
+                        m = softplus_l2(m);   // softplus * log2e
                     }
                     msum = add2(msum, m);
                     const float2 arg = mul2(m, A2);

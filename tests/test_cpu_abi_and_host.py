@@ -172,3 +172,30 @@ def test_dwconv2d_has_no_cpu_path():
         DWConv2dFn.apply(torch.randn(1, 4, 5, 5), conv.weight, conv.bias, True)
     with pytest.raises(RuntimeError, match="weight"):
         DWConv2dFn.apply(torch.randn(1, 4, 5, 5), torch.randn(4, 1, 5, 5), None, True)
+
+
+def test_model_regime_generator_and_oracles_agree():
+    """The `model` regime of tests/test_scan_ranges_gpu.py lands where it claims (softplus argument within [-9, 0], A within
+    [-32, -0.5]: what SS2D / the ARM mixers initialise), and there the two oracles - the reference's own arithmetic in fp32
+    (oracle/selective_scan_ref.py, torch autograd) and the fp64 C restatement (oracle/ss_ref.c) - agree at fp32 level on the
+    output, the last state and every gradient: the oracle is pinned in the range before it judges the kernels there."""
+    from oracle import ss_ref_c
+    from oracle.selective_scan_ref import selective_scan_ref_fwd_bwd
+    from tests.parity import cmp_f32
+    from tests.test_scan_ranges_gpu import range_inputs
+    for has_bias, has_z, N, G, ddim in ((True, False, 1, 2, 8), (False, True, 16, 1, 8), (True, True, 4, 2, 2)):
+        c = range_inputs("model", 50, 2, 8, 197, N, G, ddim, True, has_z, has_bias, True, torch.float32)
+        x = c["delta"] + (c["delta_bias"].view(1, -1, 1) if has_bias else 0.0)
+        q01, q99 = torch.quantile(x.flatten(), torch.tensor([0.01, 0.99])).tolist()
+        assert -9.0 <= q01 and q99 <= 0.0, (q01, q99)
+        assert c["A"].min() >= -32.0 and c["A"].max() <= -0.5
+        args = (c["u"], c["delta"], c["A"], c["B"], c["C"], c["D"], c["z"], c["delta_bias"])
+        ref32 = selective_scan_ref_fwd_bwd(*args, True, c["dout"])
+        r_out, r_out_z, r_last = ss_ref_c.fwd(*args, True)
+        ref64 = ss_ref_c.bwd(*args, c["dout"], True)
+        tag = f"[oracles, model regime, bias{int(has_bias)} z{int(has_z)} N{N}] "
+        cmp_f32(ref32["out"], r_out_z if has_z else r_out, tag + "out")
+        cmp_f32(ref32["last_state"], r_last, tag + "last_state")
+        for name in ("du", "ddelta", "dA", "dB", "dC", "dD", "ddelta_bias", "dz"):
+            if ref64[name] is not None:
+                cmp_f32(ref32[name], ref64[name], tag + name)

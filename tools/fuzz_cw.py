@@ -3,7 +3,10 @@
 cross-family consistency check on many geometries (rows per tensor-map row 1 / 2 / 4, split groups, partial windows, groups,
 flags), not a parity test -- those are in tests/.
 
-    python tools/bwd_variants.py --build && python tools/fuzz_cw.py [n_cases] [seed]
+    python tools/bwd_variants.py --build && python tools/fuzz_cw.py [n_cases] [seed] [--regime model]
+
+--regime model draws the inputs from the `model` regime of tests/test_scan_ranges_gpu.py (softplus argument in about [-8, -1],
+A = -(1 .. d_state) scaled per row: what SS2D / the ARM mixers initialise) instead of the reference's generators.
 """
 import json
 import os
@@ -24,8 +27,16 @@ def main():
     from medical_image_analysis_b200 import _lib
     _lib.LIB_PATH = os.path.join(ROOT, "medical_image_analysis_b200", "libmia_scan_dbg.so")
     from medical_image_analysis_b200 import scan_bwd, scan_fwd
-    n_cases = int(sys.argv[1]) if len(sys.argv) > 1 else 60
-    rng = random.Random(int(sys.argv[2]) if len(sys.argv) > 2 else 0)
+    argv = sys.argv[1:]
+    regime = None
+    if "--regime" in argv:
+        i = argv.index("--regime")
+        regime = argv[i + 1]
+        del argv[i:i + 2]
+        assert regime == "model", "--regime takes: model"
+        from tests.test_scan_ranges_gpu import range_inputs, to_gpu
+    n_cases = int(argv[0]) if len(argv) > 0 else 60
+    rng = random.Random(int(argv[1]) if len(argv) > 1 else 0)
     worst = {}
     bad = 0
     for case in range(n_cases):
@@ -46,6 +57,11 @@ def main():
         Dv = torch.randn(D, device="cuda", generator=g) if has_D else None
         bias = 0.5 * torch.rand(D, device="cuda", generator=g) if has_bias else None
         dout = torch.randn(B, D, L, device="cuda", generator=g).to(torch.float32 if (of32 or dt == torch.float32) else dt)
+        if regime == "model":
+            softplus = True
+            m = to_gpu(range_inputs("model", case, B, D, L, 1, G, D, has_D, False, has_bias, True, dt))
+            u, delta, A, Bm, Cm, Dv, bias = m["u"], m["delta"], m["A"], m["B"], m["C"], m["D"], m["delta_bias"]
+            dout = m["dout"].to(dout.dtype)
         for k in ("MIA_NO_CW_FWD", "MIA_FORCE_CW_FWD", "MIA_FORCE_CW_BWD", "MIA_NO_CW_BWD"):
             os.environ.pop(k, None)
         os.environ["MIA_FORCE_CW_FWD"] = "1"
