@@ -398,21 +398,7 @@ bool plan_cw_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::CwFwdArgs &r
     const bool of32 = eo == 4 && es != 4;
     const int tile_i = 32 * mia::kCwTok * es, tile_o = 32 * mia::kCwTok * eo;
     r.stage_bytes = 2 * tile_i;
-    // stages: 4 unless 3 gives a better-balanced last round (more resident warps)
-    int best_ns = 0, best_per_sm = 0;
-    double best_eff = -1.0;
-    for (int ns = 4; ns >= 3; --ns) {
-        const int smem = ns * r.stage_bytes + (of32 ? 2 * tile_o : 0) + 2 * mia::kCwTok * 4 + 8 * ns + 16;
-        int per_sm = (227 * 1024) / (smem + 1024);
-        if (per_sm > 16) per_sm = 16;
-        if (per_sm < 1) continue;
-        const long long slots = (long long)di.sms * per_sm;
-        const long long rounds = (n_items + slots - 1) / slots;
-        const double eff = (double)n_items / (double)(rounds * slots) * (per_sm >= 8 ? 1.0 : per_sm / 8.0);
-        if (eff > best_eff + 0.03) { best_eff = eff; best_ns = ns; best_per_sm = per_sm; }
-    }
-    if (!best_ns) return false;
-    r.ns = dbg_int("MIA_CW_STAGES", best_ns);
+    r.ns = dbg_int("MIA_CW_STAGES", 3);                          // 3 stages, at most 6 resident warps per SM: see below
     r.off_out = r.ns * r.stage_bytes;
     r.off_bc32 = r.off_out + (of32 ? 2 * tile_o : 0);
     r.off_bar = r.off_bc32 + 2 * mia::kCwTok * 4;
@@ -426,14 +412,16 @@ bool plan_cw_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::CwFwdArgs &r
         const int trc = mia::tma_make_2d(&tm[i], ptrs[i], trows, tcols, tcols * e, 32, mia::kCwTok, e, mia::kCwTok * e);
         if (trc != 0) { MIA_TRACE("cw fwd: tensor map %d rejected (CUresult %d)", i, trc); return false; }
     }
+    // At most 6 resident warps per SM.  The kernel is bound by DRAM, not by issue, and fewer concurrent row streams per SM move
+    // its bytes faster: on an H100 (80GB HBM3, 700 W; bf16, R = 3072; debug-build knobs MIA_CW_STAGES / MIA_CW_MAXPERSM) 3 stages at 6 warps take 0.214 ms at B = 132, L = 196 and
+    // 0.831 ms at B = 16, L = 6400, against 0.241 / 0.866 ms for 4 stages at 13 warps; 8 warps: 0.223 / 0.830 ms, 4 warps:
+    // 0.225 / 0.876 ms, 2 stages: >= 0.232 / 0.926 ms, 4-10 stages at 6 warps: 0.225-0.235 / 0.856-0.885 ms.
     int per_sm = (227 * 1024) / (r.smem_bytes + 1024);
-    if (per_sm > 16) per_sm = 16;
-    per_sm = std::min(per_sm, dbg_int("MIA_CW_MAXPERSM", per_sm));
+    per_sm = std::min(per_sm, dbg_int("MIA_CW_MAXPERSM", 6));
     if (per_sm < 1) return false;
     const long long slots = (long long)di.sms * per_sm;
     const long long rounds = (n_items + slots - 1) / slots;
     grid = (int)((n_items + rounds - 1) / rounds);              // equal rounds per CTA
-    (void)best_per_sm;
     return true;
 }
 
@@ -611,10 +599,7 @@ bool plan_cw_bwd(const mia_ss_params &p, const DeviceInfo &di, mia::CwBwdArgs &r
     r.nwin = (g * L + mia::kCwWin - 1) / mia::kCwWin;
     const int tile_i = 32 * mia::kCwWin * es, tile_o = 32 * mia::kCwWin * eo;
     r.stage_bytes = 2 * tile_i + tile_o;
-    // Many short rows (at least two rounds of items at 8 per SM) take 3 stages; otherwise 2 stages with the half-step-early
-    // refill (on an H100 the two are within 1 % of each other at 8 warps per SM, see below)
-    const bool many_short = L <= 256 && r.n_items >= 2LL * 8 * di.sms;
-    r.ns = dbg_int("MIA_CW_STAGES", many_short ? 3 : 2);
+    r.ns = dbg_int("MIA_CW_STAGES", 4);                          // 4 stages, at most 4 resident warps per SM: see below
     r.off_bc32 = r.ns * r.stage_bytes;
     r.off_pf = r.off_bc32 + 2 * mia::kCwWin * 4;                // two 512-byte prefetch slots (raw B, raw C, block states of 2 groups)
     r.off_red = r.off_pf + 1024;                                // [32][20] fp32 scratch of the row reductions
@@ -630,11 +615,15 @@ bool plan_cw_bwd(const mia_ss_params &p, const DeviceInfo &di, mia::CwBwdArgs &r
         if (trc != 0) { MIA_TRACE("cw bwd: tensor map %d rejected (CUresult %d)", i, trc); return false; }
     }
     int per_sm = (227 * 1024) / (r.smem_bytes + 1024);
-    // At most 8 resident warps per SM, on the build that may use 255 registers: on an H100 (80GB HBM3, 700 W; tools/bwd_variants.py,
+    // At most 4 resident warps per SM, on the build that may use 255 registers.  On an H100 (80GB HBM3, 700 W; tools/bwd_variants.py,
     // bf16, R = 3072) 8 warps beat 12 on the 168-register build wherever they differ - B = 16, L = 6400: 1.39 against 1.71 ms;
-    // B = 64, L = 196: 0.21 against 0.30 ms; B = 8, L = 1024: 0.136 against 0.144 ms - and tie at B = 132, L = 196 (0.45 ms).
-    // sm_90 issues the float2 arithmetic as two scalar instructions, so the registers buy more than the extra warps do.
-    const int cap = dbg_int("MIA_CW_MAXPERSM", 8);
+    // B = 64, L = 196: 0.21 against 0.30 ms; B = 8, L = 1024: 0.136 against 0.144 ms: sm_90 issues the float2 arithmetic as two
+    // scalar instructions, so the registers buy more than the extra warps do.  Below 8 the kernel is bound by DRAM, not by issue,
+    // and fewer concurrent row streams per SM with a deeper ring move its bytes faster (same card and knobs): 4 stages at 4 warps take
+    // 0.418 ms at B = 132, L = 196 and 1.340 ms at B = 16, L = 6400, against 0.448 / 1.405 ms for 3 / 2 stages at 8 warps;
+    // 3 stages at 4 warps: 0.413 / 1.388 ms; 2 stages: 0.445 / 1.542 ms; 5-8 stages at 4 warps: 0.417 / 1.341 ms; 3 warps:
+    // >= 0.496 / 1.729 ms; 4 stages at 5-8 warps (smem allows 7): 0.429-0.461 / 1.346-1.458 ms.
+    const int cap = dbg_int("MIA_CW_MAXPERSM", 4);
     if (per_sm > cap) per_sm = cap;
     if (per_sm < 1) return false;
     // at most 8 resident warps per SM: the build that may use 255 registers (scan_bwd_cw.cuh, kMinBlk); same results

@@ -4,13 +4,16 @@
 // Why another backward: scan_bwd_rows.cuh needs 168 registers per thread (seven 16-token
 // quantities kept from the recompute to the suffix loop) and still spills, a two-warp
 // barrier, ~170 instructions of 8-byte cp.async pieces per window.  Here
-//   * a group (16 columns of 32 rows) of u, delta and dout is one TMA box each, through a 4-stage ring: lane 0 issues three
-//     box loads per group, three groups ahead; du / ddelta replace u / delta in the stage and leave with two box stores; a
-//     stage is refilled one step after its stores were committed (cp.async.bulk.wait_group.read 1), so nobody waits;
+//   * a window (32 columns of 32 rows) of u, delta and dout is one TMA box each, through a ring of stages (4 by default):
+//     lane 0 issues three box loads per window, ns - 1 windows ahead; du / ddelta replace u / delta in the stage and leave
+//     with two box stores; a stage is refilled one step after its stores were committed (cp.async.bulk.wait_group.read 1),
+//     so nobody waits;
 //   * only a, a h_{t-1} and m (softplus) survive the recompute (48 registers instead of 112): the other per-token factors are
 //     re-derived in the suffix loop from them and from u / B, which are still in the stage; dC is reduced over the rows right
 //     after the recompute and dB after the suffix loop (two 16-value butterflies, 32 shuffles, instead of one of 32 values);
-//   * 128 registers, ~13 KB of shared memory per warp: 15-16 resident one-warp CTAs per SM, no barrier.
+//   * up to 255 registers, ~28 KB of shared memory per warp, no barrier; the planner keeps at most 4 one-warp CTAs per SM
+//     resident: the kernel is bound by DRAM, and fewer concurrent row streams with a deeper ring move its bytes faster
+//     (plan_cw_bwd).
 // Rows of 392 bytes (L = 196 bf16) are walked g = 4 (or 2) to a tensor-map row exactly like the forward, last row first (columns
 // [(g - 1) L, g L) from the end), ...; a group that holds a multiple of L is split between the two rows it touches.
 // Reductions over rows (dB, dC): the same transposing butterfly as scan_bwd_rows.cuh, one partial per (32 rows, token) in the
@@ -191,8 +194,8 @@ __device__ __forceinline__ void cw_bwd_block(const int qlo_in, const int qhi_in,
 }
 
 // kMinBlk = resident one-warp CTAs per SM the register allocation is sized for: 12 -> 168 registers (three warps per scheduler);
-// 8 -> ptxas takes 247 and has no spills: same instructions, scheduled with the loads hoisted further.  The planner runs many
-// short items with 8 warps per SM anyway (plan_cw_bwd), so that build costs them no residency.
+// 8 -> ptxas takes 247 and has no spills: same instructions, scheduled with the loads hoisted further.  The planner runs at
+// most 4 warps per SM (plan_cw_bwd), so that build costs no residency.
 template <typename T, bool kSoftplus, bool kOutF32, int kG, int kMinBlk>
 __global__ void __launch_bounds__(32, kMinBlk) ss_bwd_cw_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_d,
                                                            const __grid_constant__ CUtensorMap tm_o, const __grid_constant__ CUtensorMap tm_du,

@@ -5,12 +5,12 @@
 // buffer (load, wait, compute, store, wait) with 8 warps per SM, so every chunk exposes a full load latency, and with 13 KB
 // tiles the 1536 work items of L = 6400, B = 16 do not all fit at once.  Here
 //   * a warp owns 32 tensor-map rows and walks them in windows of 32 columns; a window of u and of delta is one box copy each
-//     (2 KB for 2-byte types), issued by lane 0 into a ring of 3-4 stages, two or three windows ahead of the one being
+//     (2 KB for 2-byte types), issued by lane 0 into a ring of stages (3 by default), two windows ahead of the one being
 //     computed; completion is an mbarrier per stage;
 //   * y replaces u in the stage and leaves with one box store; the stage is refilled one step later, when
 //     cp.async.bulk.wait_group.read says the store has been read out -- no step waits for its own store;
-//   * 12-16 KB of shared memory per warp: 13-16 resident warps per SM, and a B = 16, L = 6400 problem (1536 items) is
-//     resident all at once;
+//   * ~12 KB of shared memory per warp; the planner keeps at most 6 warps per SM resident: the kernel is bound by DRAM, and
+//     fewer concurrent row streams move its bytes faster (plan_cw_fwd);
 //   * tiles carry the TMA swizzle whose span is the tile row (64 B -> SWIZZLE_64B, 128 B -> SWIZZLE_128B): the 32 lanes read
 //     the same column of 32 different rows, which unswizzled would hit 2-4 banks.
 // Rows whose byte pitch is not a multiple of 16 (L = 196 bf16: 392 B) cannot be a tensor-map row; g = 2 or 4 consecutive rows
