@@ -3,10 +3,12 @@
 // backward's deterministic partials, and the extern "C" surface declared in include/mia_selective_scan.h.
 #include <algorithm>
 #include <atomic>
+#include <initializer_list>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "../../include/mia_selective_scan.h"
 #include "scan_common.cuh"
@@ -201,7 +203,7 @@ int validate_common(const mia_ss_params &p) {
     return MIA_OK;
 }
 
-void fill_common(mia::ScanArgs &a, const mia_ss_params &p, const Plan &pl, bool bwd) {
+void fill_common(mia::ScanArgs &a, const mia_ss_params &p, const Plan &pl) {
     memset(&a, 0, sizeof(a));
     a.batch = p.batch; a.dim = p.dim; a.L = p.seqlen; a.N = p.dstate; a.G = p.n_groups; a.delta_dim = p.delta_dim;
     a.rows_per_group = p.dim / p.n_groups;
@@ -221,7 +223,6 @@ void fill_common(mia::ScanArgs &a, const mia_ss_params &p, const Plan &pl, bool 
     a.flat_z = a.has_z && whole && p.z_d_stride == p.seqlen;
     a.flat_B = whole && p.B_dstate_stride == p.seqlen;
     a.flat_C = whole && p.C_dstate_stride == p.seqlen;
-    (void)bwd;
 }
 
 // Shared-memory carve-up.  Returns false if not even two row stages fit.  det: also the tickets and (det_acc, and 2 N CH
@@ -253,11 +254,10 @@ bool layout_smem(mia::ScanArgs &a, int es, int eso, bool bwd, int smem_max, bool
     const int bars = round_up((2 * mia::kMaxStages + 2 * mia::kGroupStages) * 8, 128);
     const int carry = round_up(bwd ? (2 * a.RS * a.N + 2 * a.RS) * 4 : a.RS * a.N * 8, 128);
     const int red = bwd ? a.n_consumer_warps * 256 * 4 : 0;
-    const int bcf = 0;   // (an fp32 copy of the B / C chunk for the d_state > 1 fast backward was tried and removed)
     const int tickets = round_up(2 * a.N * 4, 128);
     a.det_smem_acc = det && det_acc && 2 * a.N * a.CH * 4 <= 32768;
     const int det_bytes = det ? tickets + (a.det_smem_acc ? 2 * a.N * a.CH * 4 : 0) : 0;
-    const int fixed = mia::kGroupStages * a.gstage_bytes + bars + carry + red + bcf + det_bytes;
+    const int fixed = mia::kGroupStages * a.gstage_bytes + bars + carry + red + det_bytes;
     int stages = (smem_max - fixed) / a.stage_bytes;
     if (stages > mia::kMaxStages) stages = mia::kMaxStages;
     if (stages < 2) return false;
@@ -266,8 +266,7 @@ bool layout_smem(mia::ScanArgs &a, int es, int eso, bool bwd, int smem_max, bool
     a.off_bars = a.off_groups + mia::kGroupStages * a.gstage_bytes;
     a.off_carry = a.off_bars + bars;
     a.off_red = a.off_carry + carry;
-    a.off_bcf = bcf ? a.off_red + red : 0;
-    a.smem_bytes = a.off_red + red + bcf;
+    a.smem_bytes = a.off_red + red;
     if (det) {
         a.off_det = a.smem_bytes;
         a.off_det_acc = a.off_det + tickets;
@@ -284,7 +283,7 @@ int plan_and_layout(const mia_ss_params &p, const DeviceInfo &di, bool bwd, Plan
     const int es = esize(p.itype), eso = esize(p.otype);
     const int rpg = p.dim / p.n_groups;
     for (;;) {
-        fill_common(a, p, pl, bwd);
+        fill_common(a, p, pl);
         if (bwd) {
             const bool whole = pl.n_chunks == 1;
             a.flat_dout = whole && p.dout_d_stride == p.seqlen;
@@ -304,6 +303,60 @@ int plan_and_layout(const mia_ss_params &p, const DeviceInfo &di, bool bwd, Plan
     }
 }
 
+// Eligibility checks shared by the planners below.  Each plan_* states only what is particular to its family.
+struct RowStrides { long long bs, ds; };   // one (batch, dim, L) operand: batch and row strides in elements
+#define MIA_ROWS(t) RowStrides{p.t##_batch_stride, p.t##_d_stride}
+
+// The operands are dense (batch, dim, L) rows: rows L elements apart, batches dim L apart.
+bool dense_rows(const mia_ss_params &p, std::initializer_list<RowStrides> ops) {
+    for (const RowStrides &o : ops)
+        if (o.ds != p.seqlen || o.bs != (long long)p.dim * p.seqlen) return false;
+    return true;
+}
+
+// Every pointer is a multiple of `bytes` (a power of two).
+bool aligned(uintptr_t bytes, std::initializer_list<const void *> ptrs) {
+    uintptr_t bits = 0;
+    for (const void *q : ptrs) bits |= (uintptr_t)q;
+    return (bits & (bytes - 1)) == 0;
+}
+
+// What every d_state 1 row-serial kernel needs: one delta row per row, no gate, whole 32-row batches in a group, rows of
+// whole 4-token pieces.
+bool rowwise_n1(const mia_ss_params &p) {
+    return p.dstate == 1 && !p.z && p.delta_dim == p.dim && (p.dim / p.n_groups) % 32 == 0 && p.seqlen % 4 == 0;
+}
+
+// The d_state 1 row-serial kernels read A as one float per row.
+bool a_per_row(const mia_ss_params &p) { return p.A_d_stride == 1 || p.dim == 1; }
+
+// Shared memory per SM as the planners count it: the 227 KB one CTA may opt in to.
+constexpr int kSmemPerSm = 227 * 1024;
+
+// Grid of a persistent kernel: as many CTAs per SM as `capacity` bytes of shared memory hold at `smem` bytes each (plus the
+// 1 KB the SM reserves per CTA), at most hi, on every SM, at most one per item; 0 when fewer than lo fit (the family declines).
+int resident_grid(const DeviceInfo &di, int smem, int capacity, int lo, int hi, int n_items) {
+    const int per_sm = std::min(capacity / (smem + 1024), hi);
+    return per_sm < lo ? 0 : std::min(di.sms * per_sm, n_items);
+}
+
+template <typename R, typename = void> struct HasRows : std::false_type {};
+template <typename R> struct HasRows<R, std::void_t<decltype(R::u)>> : std::true_type {};
+template <typename R, typename = void> struct HasOut : std::false_type {};
+template <typename R> struct HasOut<R, std::void_t<decltype(R::out)>> : std::true_type {};
+
+// Zero a row-serial or column-walk argument block and fill the fields they all share.
+template <typename R>
+void fill_rows_common(R &r, const mia_ss_params &p) {
+    memset(&r, 0, sizeof(r));
+    r.batch = p.batch; r.dim = p.dim; r.L = p.seqlen; r.G = p.n_groups; r.rows_per_group = p.dim / p.n_groups;
+    r.softplus = p.delta_softplus;
+    r.A = p.A; r.B = p.B; r.C = p.C; r.D = p.D; r.delta_bias = p.delta_bias;
+    r.B_bs = p.B_batch_stride; r.B_gs = p.B_group_stride; r.C_bs = p.C_batch_stride; r.C_gs = p.C_group_stride;
+    if constexpr (HasRows<R>::value) { r.u = p.u; r.delta = p.delta; }
+    if constexpr (HasOut<R>::value) r.out = p.out;
+}
+
 // Geometry of the column-walk kernels (scan_fwd_cw.cuh / scan_bwd_cw.cuh): g rows per tensor-map row.  A pure function of the
 // problem's sizes and dtypes (and the SM count) -- it also fixes the LAYOUT of the block states (hblk), which forward and backward must agree on.
 // A tensor-map row must be a multiple of 16 bytes (else the map cannot be encoded); it SHOULD be a multiple of 32 (else every
@@ -314,9 +367,9 @@ int plan_and_layout(const mia_ss_params &p, const DeviceInfo &di, bool bwd, Plan
 // lane).  fp32 rows (L % 4 == 0) are always legal: g = 1.
 bool cw_geometry(const mia_ss_params &p, int sms, int &g) {
     const int es = esize(p.itype), L = p.seqlen;
-    if (p.dstate != 1 || p.z || p.delta_dim != p.dim || (L % 4) || p.n_groups < 1) return false;
+    if (!rowwise_n1(p)) return false;
     const int rpg = p.dim / p.n_groups;
-    if (es == 4) { g = 1; return rpg % 32 == 0; }
+    if (es == 4) { g = 1; return true; }
     const int want = (L % 16 == 0) ? 1 : (L % 8 == 0) ? 2 : 4;
     // Items are 32 g rows: a larger g halves their number, and a problem that fills the resident slots a little more than once
     // pays a whole second round -> take the preferred g when its items fit one round or make at least two, else the next smaller
@@ -339,36 +392,27 @@ bool cw_geometry(const mia_ss_params &p, int sms, int &g) {
 // Row-serial forward (scan_fwd_rows.cuh): eligibility + argument block.  Returns false when the warp-scan kernels must run.
 bool plan_rows_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::RowsArgs &r, int &grid) {
     const int es = esize(p.itype), L = p.seqlen;
-    const int rpg = p.dim / p.n_groups;
-    if (p.dstate != 1 || p.z || p.delta_dim != p.dim || (rpg % 32) || (L % 4)) return false;
+    if (!rowwise_n1(p)) return false;
     if (dbg_knob("MIA_NO_ROWS_FWD")) return false;
-    auto dense = [&](long long bs, long long ds) { return ds == L && bs == (long long)p.dim * L; };
-    if (!dense(p.u_batch_stride, p.u_d_stride) || !dense(p.delta_batch_stride, p.delta_d_stride) ||
-        !dense(p.out_batch_stride, p.out_d_stride)) return false;
-    if (p.A_d_stride != 1 && p.dim > 1) return false;
-    if (((uintptr_t)p.u | (uintptr_t)p.delta | (uintptr_t)p.out) & 15) return false;
-    memset(&r, 0, sizeof(r));
+    if (!dense_rows(p, {MIA_ROWS(u), MIA_ROWS(delta), MIA_ROWS(out)}) || !a_per_row(p) || !aligned(16, {p.u, p.delta, p.out})) return false;
     const int budget = 13 * 1024;                               // bytes of one [32 x chunk] tile (8 warps per SM at 2-byte dtypes)
     int Lc = L;
     if (32 * L * es > budget) {
         if ((L * es) % 16) return false;                        // per-row pieces must start 16-byte aligned
         Lc = budget / (32 * es) / 8 * 8;
     }
-    r.batch = p.batch; r.dim = p.dim; r.L = L; r.G = p.n_groups; r.rows_per_group = rpg; r.softplus = p.delta_softplus;
+    fill_rows_common(r, p);
     r.Lc = Lc; r.n_lchunks = (L + Lc - 1) / Lc;
-    r.n_items = p.batch * p.n_groups * (rpg / 32);
+    r.n_items = p.batch * p.n_groups * (r.rows_per_group / 32);
     r.tile_bytes = round_up(32 * Lc * es, 128);
-    r.bc_bytes = 0;
     r.off_bc32 = 2 * r.tile_bytes;
     r.stage_bytes = r.off_bc32 + round_up(2 * Lc * 4, 128);
     r.smem_bytes = r.stage_bytes + 128;
     if (r.smem_bytes > di.smem_optin) return false;
     r.xchunks = mia_ss_num_chunks(L); r.xchunk_tokens = mia_ss_chunk_len(L);
-    r.u = p.u; r.delta = p.delta; r.A = p.A; r.B = p.B; r.C = p.C; r.D = p.D; r.delta_bias = p.delta_bias; r.out = p.out; r.x = p.x;
-    r.B_bs = p.B_batch_stride; r.B_gs = p.B_group_stride; r.C_bs = p.C_batch_stride; r.C_gs = p.C_group_stride;
-    const int per_sm = di.smem_optin / (r.smem_bytes + 1024) > 0 ? (227 * 1024) / (r.smem_bytes + 1024) : 1;
-    grid = di.sms * (per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm));
-    if (grid > r.n_items) grid = r.n_items;
+    r.x = p.x;
+    grid = di.smem_optin / (r.smem_bytes + 1024) > 0 ? resident_grid(di, r.smem_bytes, kSmemPerSm, 1, 8, r.n_items) : 0;
+    if (!grid) grid = std::min(di.sms, r.n_items);              // a tile that leaves no room for the 1 KB reserve: one per SM
     return true;
 }
 
@@ -378,20 +422,14 @@ bool plan_cw_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::CwFwdArgs &r
     int g = 0;
     if (!cw_geometry(p, di.sms, g)) return false;
     if (dbg_knob("MIA_NO_CW_FWD")) return false;
-    const int rpg = p.dim / p.n_groups;
-    auto dense = [&](long long bs, long long ds) { return ds == L && bs == (long long)p.dim * L; };
-    if (!dense(p.u_batch_stride, p.u_d_stride) || !dense(p.delta_batch_stride, p.delta_d_stride) ||
-        !dense(p.out_batch_stride, p.out_d_stride)) return false;
-    if (p.A_d_stride != 1 && p.dim > 1) return false;
-    if (((uintptr_t)p.u | (uintptr_t)p.delta | (uintptr_t)p.out) & 15) return false;
+    if (!dense_rows(p, {MIA_ROWS(u), MIA_ROWS(delta), MIA_ROWS(out)}) || !a_per_row(p) || !aligned(16, {p.u, p.delta, p.out})) return false;
     const unsigned long long trows = (unsigned long long)p.batch * p.dim / g, tcols = (unsigned long long)g * L;
     if (tcols >= (1ull << 31) || trows >= (1ull << 31)) return false;
-    const int n_items = p.batch * p.n_groups * (rpg / (32 * g));
+    const int n_items = p.batch * p.n_groups * (p.dim / p.n_groups / (32 * g));
     // few long rows: the chunk-parallel kernel (scan_fwd_chunks.cuh) has more warps to offer than one per 32 rows
     if (n_items < 4 * di.sms && (L + mia::kChunkTok - 1) / mia::kChunkTok >= 2 && !dbg_knob("MIA_FORCE_CW_FWD")) return false;
-    memset(&r, 0, sizeof(r));
+    fill_rows_common(r, p);
     r.zero = 0;                                                  // (the kernel XORs parameter loads with it: scan_fwd_cw.cuh, settle)
-    r.batch = p.batch; r.dim = p.dim; r.L = L; r.G = p.n_groups; r.rows_per_group = rpg; r.softplus = p.delta_softplus;
     r.g = g; r.n_items = n_items;
     r.nwin = (g * L + mia::kCwTok - 1) / mia::kCwTok;
     r.ngrp = (g * L + 15) / 16;
@@ -404,8 +442,7 @@ bool plan_cw_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::CwFwdArgs &r
     r.off_bar = r.off_bc32 + 2 * mia::kCwTok * 4;
     r.smem_bytes = r.off_bar + 8 * r.ns + 16;
     r.xchunks = mia_ss_num_chunks(L); r.xchunk_tokens = mia_ss_chunk_len(L);
-    r.A = p.A; r.B = p.B; r.C = p.C; r.D = p.D; r.delta_bias = p.delta_bias; r.x = p.x; r.hblk = p.hblk;
-    r.B_bs = p.B_batch_stride; r.B_gs = p.B_group_stride; r.C_bs = p.C_batch_stride; r.C_gs = p.C_group_stride;
+    r.x = p.x; r.hblk = p.hblk;
     const void *ptrs[3] = {p.u, p.delta, p.out};
     for (int i = 0; i < 3; ++i) {
         const int e = i == 2 ? eo : es;
@@ -416,78 +453,54 @@ bool plan_cw_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::CwFwdArgs &r
     // its bytes faster: on an H100 (80GB HBM3, 700 W; bf16, R = 3072; debug-build knobs MIA_CW_STAGES / MIA_CW_MAXPERSM) 3 stages at 6 warps take 0.214 ms at B = 132, L = 196 and
     // 0.831 ms at B = 16, L = 6400, against 0.241 / 0.866 ms for 4 stages at 13 warps; 8 warps: 0.223 / 0.830 ms, 4 warps:
     // 0.225 / 0.876 ms, 2 stages: >= 0.232 / 0.926 ms, 4-10 stages at 6 warps: 0.225-0.235 / 0.856-0.885 ms.
-    int per_sm = (227 * 1024) / (r.smem_bytes + 1024);
-    per_sm = std::min(per_sm, dbg_int("MIA_CW_MAXPERSM", 6));
-    if (per_sm < 1) return false;
-    const long long slots = (long long)di.sms * per_sm;
-    const long long rounds = (n_items + slots - 1) / slots;
-    grid = (int)((n_items + rounds - 1) / rounds);              // equal rounds per CTA
+    const int fill = resident_grid(di, r.smem_bytes, kSmemPerSm, 1, dbg_int("MIA_CW_MAXPERSM", 6), n_items);
+    if (!fill) return false;
+    const int rounds = (n_items + fill - 1) / fill;
+    grid = (n_items + rounds - 1) / rounds;                      // equal rounds per CTA
     return true;
 }
 
 // Chunk-parallel forward for long rows and few 32-row batches (scan_fwd_chunks.cuh): eligibility + argument block.
 bool plan_chunks_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::ChunkArgs &r, int &grid) {
     const int es = esize(p.itype), eo = esize(p.otype), L = p.seqlen;
-    const int rpg = p.dim / p.n_groups;
-    if (p.dstate != 1 || p.z || p.delta_dim != p.dim || (rpg % 32) || (L % 4)) return false;
+    if (!rowwise_n1(p)) return false;
     if (dbg_knob("MIA_NO_ROWS_FWD") || dbg_knob("MIA_NO_CHUNKS_FWD")) return false;
     const int nch = (L + mia::kChunkTok - 1) / mia::kChunkTok;
     if (nch < 2 || mia_ss_chunk_len(L) != mia::kChunkTok || ((L * es) % 16) || ((L * eo) % 16)) return false;
-    const int n_batches = p.batch * p.n_groups * (rpg / 32);
+    const int n_batches = p.batch * p.n_groups * (p.dim / p.n_groups / 32);
     if (n_batches >= 4 * di.sms) return false;                 // enough rows: the serial row walk fills the machine
-    auto dense = [&](long long bs, long long ds) { return ds == L && bs == (long long)p.dim * L; };
-    if (!dense(p.u_batch_stride, p.u_d_stride) || !dense(p.delta_batch_stride, p.delta_d_stride) ||
-        !dense(p.out_batch_stride, p.out_d_stride)) return false;
-    if (p.A_d_stride != 1 && p.dim > 1) return false;
-    if (((uintptr_t)p.u | (uintptr_t)p.delta | (uintptr_t)p.out) & 15) return false;
-    memset(&r, 0, sizeof(r));
-    r.batch = p.batch; r.dim = p.dim; r.L = L; r.G = p.n_groups; r.rows_per_group = rpg; r.softplus = p.delta_softplus;
+    if (!dense_rows(p, {MIA_ROWS(u), MIA_ROWS(delta), MIA_ROWS(out)}) || !a_per_row(p) || !aligned(16, {p.u, p.delta, p.out})) return false;
+    fill_rows_common(r, p);
     r.n_chunks = nch;
     r.n_items = n_batches * nch;
     r.tile_bytes = round_up(32 * (mia::kChunkTok * es + 16), 128);
     r.off_bc32 = 2 * r.tile_bytes;
     r.off_bar = r.off_bc32 + 2 * mia::kChunkTok * 4;
     r.smem_bytes = r.off_bar + 128;
-    int per_sm = (227 * 1024) / (r.smem_bytes + 1024);
-    if (per_sm < 3) return false;
-    if (per_sm > 8) per_sm = 8;
-    r.u = p.u; r.delta = p.delta; r.A = p.A; r.B = p.B; r.C = p.C; r.D = p.D; r.delta_bias = p.delta_bias; r.out = p.out; r.x = p.x;
-    r.B_bs = p.B_batch_stride; r.B_gs = p.B_group_stride; r.C_bs = p.C_batch_stride; r.C_gs = p.C_group_stride;
-    grid = di.sms * per_sm;
-    if (grid > r.n_items) grid = r.n_items;
-    return true;
+    r.x = p.x;
+    grid = resident_grid(di, r.smem_bytes, kSmemPerSm, 3, 8, r.n_items);
+    return grid > 0;
 }
 
 // Streaming row-serial forward (scan_fwd_stream.cuh): eligibility + argument block.
 bool plan_stream_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::StreamArgs &r, int &grid) {
     const int es = esize(p.itype), eo = esize(p.otype), L = p.seqlen;
-    const int rpg = p.dim / p.n_groups;
-    if (p.dstate != 1 || p.z || p.delta_dim != p.dim || (rpg % 32) || (L % 4)) return false;
+    if (!rowwise_n1(p)) return false;
     if (dbg_knob("MIA_NO_ROWS_FWD") || dbg_knob("MIA_NO_STREAM_FWD")) return false;
-    auto dense = [&](long long bs, long long ds) { return ds == L && bs == (long long)p.dim * L; };
-    if (!dense(p.u_batch_stride, p.u_d_stride) || !dense(p.delta_batch_stride, p.delta_d_stride) ||
-        !dense(p.out_batch_stride, p.out_d_stride)) return false;
-    if (p.A_d_stride != 1 && p.dim > 1) return false;
-    const uintptr_t piece = 4 * es - 1, pieceo = 4 * eo - 1;    // every row start is a multiple of one 4-token piece
-    if ((((uintptr_t)p.u | (uintptr_t)p.delta) & piece) || ((uintptr_t)p.out & pieceo)) return false;
+    if (!dense_rows(p, {MIA_ROWS(u), MIA_ROWS(delta), MIA_ROWS(out)}) || !a_per_row(p)) return false;
+    if (!aligned(4 * es, {p.u, p.delta}) || !aligned(4 * eo, {p.out})) return false;   // every row start is a multiple of one 4-token piece
     if (L > 256 && mia_ss_chunk_len(L) != 256) return false;
-    memset(&r, 0, sizeof(r));
-    r.batch = p.batch; r.dim = p.dim; r.L = L; r.G = p.n_groups; r.rows_per_group = rpg; r.softplus = p.delta_softplus;
-    r.n_items = p.batch * p.n_groups * (rpg / 32);
+    fill_rows_common(r, p);
+    r.n_items = p.batch * p.n_groups * (r.rows_per_group / 32);
     r.Lp = (L + 3) & ~3;
     const int pitch = mia::kStreamTok * es + 4 * es;
     r.off_bc32 = round_up(2 * 2 * 32 * pitch, 128);             // 2 stages x (u, delta)
     r.smem_bytes = r.off_bc32 + round_up(2 * r.Lp * 4, 128);
     if (r.smem_bytes > di.smem_optin) return false;
     r.xchunks = mia_ss_num_chunks(L);
-    r.u = p.u; r.delta = p.delta; r.A = p.A; r.B = p.B; r.C = p.C; r.D = p.D; r.delta_bias = p.delta_bias; r.out = p.out; r.x = p.x;
-    r.B_bs = p.B_batch_stride; r.B_gs = p.B_group_stride; r.C_bs = p.C_batch_stride; r.C_gs = p.C_group_stride;
-    int per_sm = (227 * 1024) / (r.smem_bytes + 1024);
-    if (per_sm > 16) per_sm = 16;                               // 128 registers per thread
-    if (per_sm < 4) return false;
-    grid = di.sms * per_sm;
-    if (grid > r.n_items) grid = r.n_items;
-    return true;
+    r.x = p.x;
+    grid = resident_grid(di, r.smem_bytes, kSmemPerSm, 4, 16, r.n_items);   // at most 16: 128 registers per thread
+    return grid > 0;
 }
 
 // Row-serial forward for d_state > 1 (scan_fwd_rowsn.cuh): eligibility + argument block.
@@ -497,15 +510,11 @@ bool plan_rowsn_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::RowsNArgs
     if ((N != 16 && N != 8) || p.delta_dim != p.dim || (rpg % 32)) return false;
     if (dbg_knob("MIA_NO_ROWS_FWD")) return false;
     if (mia_ss_num_chunks(L) != 1) return false;                // whole rows, one checkpoint
-    auto dense = [&](long long bs, long long ds) { return ds == L && bs == (long long)p.dim * L; };
-    if (!dense(p.u_batch_stride, p.u_d_stride) || !dense(p.delta_batch_stride, p.delta_d_stride) ||
-        !dense(p.out_batch_stride, p.out_d_stride)) return false;
-    if (((uintptr_t)p.u | (uintptr_t)p.delta | (uintptr_t)p.out) & 15) return false;
-    if (p.z && (!dense(p.z_batch_stride, p.z_d_stride) || !dense(p.out_z_batch_stride, p.out_z_d_stride) ||
-                (((uintptr_t)p.z | (uintptr_t)p.out_z) & 15))) return false;
+    if (!dense_rows(p, {MIA_ROWS(u), MIA_ROWS(delta), MIA_ROWS(out)}) || !aligned(16, {p.u, p.delta, p.out})) return false;
+    if (p.z && (!dense_rows(p, {MIA_ROWS(z), MIA_ROWS(out_z)}) || !aligned(16, {p.z, p.out_z}))) return false;
     if ((32 * L * es) % 16) return false;
-    memset(&r, 0, sizeof(r));
-    r.batch = p.batch; r.dim = p.dim; r.L = L; r.G = p.n_groups; r.rows_per_group = rpg; r.N = N; r.softplus = p.delta_softplus;
+    fill_rows_common(r, p);
+    r.N = N;
     r.warps = p.z ? 2 : mia::kRowsNWarps;
     r.tiles_per_warp = p.z ? 3 : 2;
     const int W = r.warps;
@@ -515,36 +524,26 @@ bool plan_rowsn_fwd(const mia_ss_params &p, const DeviceInfo &di, mia::RowsNArgs
     r.off_bc = W * r.tiles_per_warp * r.tile_bytes;
     r.off_bar = r.off_bc + round_up(2 * L * N * es, 128);
     r.smem_bytes = r.off_bar + 128;
-    const int per_sm = (int)(233472 / (r.smem_bytes + 1024));
-    if (per_sm < 1 || r.smem_bytes > di.smem_optin) return false;
-    r.u = p.u; r.delta = p.delta; r.A = p.A; r.B = p.B; r.C = p.C; r.D = p.D; r.delta_bias = p.delta_bias; r.out = p.out; r.x = p.x;
-    r.z = p.z; r.out_z = p.out_z;
-    r.A_ds = p.A_d_stride; r.A_ns = p.A_dstate_stride;
-    r.B_bs = p.B_batch_stride; r.B_gs = p.B_group_stride; r.B_ns = p.B_dstate_stride;
-    r.C_bs = p.C_batch_stride; r.C_gs = p.C_group_stride; r.C_ns = p.C_dstate_stride;
-    grid = di.sms * (per_sm > 4 ? 4 : per_sm);
-    if (grid > r.n_units) grid = r.n_units;
-    return true;
+    if (r.smem_bytes > di.smem_optin) return false;
+    r.x = p.x; r.z = p.z; r.out_z = p.out_z;
+    r.A_ds = p.A_d_stride; r.A_ns = p.A_dstate_stride; r.B_ns = p.B_dstate_stride; r.C_ns = p.C_dstate_stride;
+    // This family counts the SM's whole 228 KB, not kSmemPerSm: counting 227 KB would change its grid at some sizes.
+    grid = resident_grid(di, r.smem_bytes, 228 * 1024, 1, 4, r.n_units);
+    return grid > 0;
 }
 
 // Row-serial backward (scan_bwd_rows.cuh): eligibility + argument block.  Returns false when the warp-scan kernels must run.
 bool plan_rows_bwd(const mia_ss_params &p, const DeviceInfo &di, mia::RowsBwdArgs &r, int &grid) {
     const int es = esize(p.itype), eo = esize(p.otype), L = p.seqlen;
-    const int rpg = p.dim / p.n_groups;
-    if (p.dstate != 1 || p.z || p.delta_dim != p.dim || (rpg % 32) || (L % 4)) return false;
+    if (!rowwise_n1(p)) return false;
     if (dbg_knob("MIA_NO_ROWS_BWD")) return false;
     const int CH = mia::kRowsChunk;
     const int nch = (L + CH - 1) / CH;
     // long rows: x must hold a checkpoint every 256 tokens, and the per-row pieces of a tile must be 16-byte aligned
     if (nch > 1 && (mia_ss_chunk_len(L) != CH || !p.x || ((L * es) % 16) || ((L * eo) % 16))) return false;
-    auto dense = [&](long long bs, long long ds) { return ds == L && bs == (long long)p.dim * L; };
-    if (!dense(p.u_batch_stride, p.u_d_stride) || !dense(p.delta_batch_stride, p.delta_d_stride) ||
-        !dense(p.dout_batch_stride, p.dout_d_stride) || !dense(p.du_batch_stride, p.du_d_stride) ||
-        !dense(p.ddelta_batch_stride, p.ddelta_d_stride)) return false;
-    if (p.A_d_stride != 1 && p.dim > 1) return false;
-    if (((uintptr_t)p.u | (uintptr_t)p.delta | (uintptr_t)p.dout | (uintptr_t)p.du | (uintptr_t)p.ddelta) & 15) return false;
-    memset(&r, 0, sizeof(r));
-    r.batch = p.batch; r.dim = p.dim; r.L = L; r.G = p.n_groups; r.rows_per_group = rpg; r.softplus = p.delta_softplus;
+    if (!dense_rows(p, {MIA_ROWS(u), MIA_ROWS(delta), MIA_ROWS(dout), MIA_ROWS(du), MIA_ROWS(ddelta)}) || !a_per_row(p) ||
+        !aligned(16, {p.u, p.delta, p.dout, p.du, p.ddelta})) return false;
+    fill_rows_common(r, p);
     r.n_chunks = nch;
     const int span = nch == 1 ? L : CH;                         // tokens of a row resident at a time
     r.t0_pct = dbg_int("MIA_T0_PCT", 52);   // share of a chunk for the half that has no Gs to accumulate
@@ -552,7 +551,7 @@ bool plan_rows_bwd(const mia_ss_params &p, const DeviceInfo &di, mia::RowsBwdArg
     const int longer = T0 > span - T0 ? T0 : span - T0;
     r.nblk = (longer + mia::kBlk - 1) / mia::kBlk;
     r.Lp = (span + mia::kBlk - 1) / mia::kBlk * mia::kBlk + mia::kBlk;
-    r.n_items = p.batch * p.n_groups * (rpg / 32);
+    r.n_items = p.batch * p.n_groups * (r.rows_per_group / 32);
     r.tile_bytes = round_up(32 * (span * es + (nch > 1 ? 16 : 0)), 128);
     r.tileo_bytes = round_up(32 * (span * eo + (nch > 1 ? 16 : 0)), 128);
     r.off_delta = r.tile_bytes;
@@ -562,39 +561,32 @@ bool plan_rows_bwd(const mia_ss_params &p, const DeviceInfo &di, mia::RowsBwdArg
     r.off_xch = r.off_ck + 3 * r.nblk * 128;                    // ck of both halves + ckm
     r.off_bar = r.off_xch + 7 * 128;
     r.smem_bytes = r.off_bar + 128;
-    int per_sm = (227 * 1024) / (r.smem_bytes + 1024);
-    if (per_sm < 3) return false;                               // too few resident warps to hide the dependent chains
-    if (per_sm > 5) per_sm = 5;                                 // 64 threads x 168 registers: 3 warps per scheduler
-    r.u = p.u; r.delta = p.delta; r.A = p.A; r.B = p.B; r.C = p.C; r.D = p.D; r.delta_bias = p.delta_bias; r.dout = p.dout;
-    r.du = p.du; r.ddelta = p.ddelta; r.x = p.x;
-    r.B_bs = p.B_batch_stride; r.B_gs = p.B_group_stride; r.C_bs = p.C_batch_stride; r.C_gs = p.C_group_stride;
-    grid = di.sms * per_sm;
+    r.dout = p.dout; r.du = p.du; r.ddelta = p.ddelta; r.x = p.x;
+    // at least 3 resident CTAs to hide the dependent chains; at most 5: 64 threads x 168 registers, 3 warps per scheduler
+    grid = resident_grid(di, r.smem_bytes, kSmemPerSm, 3, 5, r.n_items);
     // Long rows: a CTA walks its 32 rows chunk by chunk and each chunk is latency-bound (load -> phase 1 -> exchange ->
     // phase 2 -> store), so this path only wins while every item gets its own resident CTA.
-    if (nch > 1 && r.n_items > grid) return false;
-    if (grid > r.n_items) grid = r.n_items;
-    return true;
+    return grid > 0 && !(nch > 1 && r.n_items > grid);
 }
 
 // Column-walk backward (scan_bwd_cw.cuh): eligibility, argument block, tensor maps (u, delta, dout, du, ddelta).
 bool plan_cw_bwd(const mia_ss_params &p, const DeviceInfo &di, mia::CwBwdArgs &r, CUtensorMap *tm, int &grid) {
     const int es = esize(p.itype), eo = esize(p.otype), L = p.seqlen;
+    // Only on the forward's block states (one warp per 32 g rows, phase 2 only).  Short rows always; rows of more than one
+    // 256-token chunk only with enough 32-row items to fill the SMs (four per SM): below that a one-warp-per-item walk leaves
+    // the SMs short of warps and the warp-scan kernel is used.
+    const long long items32 = (long long)p.batch * (p.dim / 32);
+    if (!p.hblk || !(L <= mia::kRowsChunk || items32 >= 4LL * di.sms || dbg_knob("MIA_FORCE_CW_BWD"))) return false;
     int g = 0;
-    if (!p.hblk || !cw_geometry(p, di.sms, g)) return false;
+    if (!cw_geometry(p, di.sms, g)) return false;
     if (dbg_knob("MIA_NO_CW_BWD")) return false;
-    const int rpg = p.dim / p.n_groups;
-    auto dense = [&](long long bs, long long ds) { return ds == L && bs == (long long)p.dim * L; };
-    if (!dense(p.u_batch_stride, p.u_d_stride) || !dense(p.delta_batch_stride, p.delta_d_stride) ||
-        !dense(p.dout_batch_stride, p.dout_d_stride) || !dense(p.du_batch_stride, p.du_d_stride) ||
-        !dense(p.ddelta_batch_stride, p.ddelta_d_stride)) return false;
-    if (p.A_d_stride != 1 && p.dim > 1) return false;
-    if (((uintptr_t)p.u | (uintptr_t)p.delta | (uintptr_t)p.dout | (uintptr_t)p.du | (uintptr_t)p.ddelta) & 15) return false;
+    if (!dense_rows(p, {MIA_ROWS(u), MIA_ROWS(delta), MIA_ROWS(dout), MIA_ROWS(du), MIA_ROWS(ddelta)}) || !a_per_row(p) ||
+        !aligned(16, {p.u, p.delta, p.dout, p.du, p.ddelta})) return false;
     const unsigned long long trows = (unsigned long long)p.batch * p.dim / g, tcols = (unsigned long long)g * L;
     if (tcols >= (1ull << 31) || trows >= (1ull << 31)) return false;
-    memset(&r, 0, sizeof(r));
-    r.batch = p.batch; r.dim = p.dim; r.L = L; r.G = p.n_groups; r.rows_per_group = rpg; r.softplus = p.delta_softplus;
+    fill_rows_common(r, p);
     r.g = g;
-    r.n_items = p.batch * p.n_groups * (rpg / (32 * g));
+    r.n_items = p.batch * p.n_groups * (r.rows_per_group / (32 * g));
     r.ngrp = (g * L + mia::kCwGrp - 1) / mia::kCwGrp;
     r.nwin = (g * L + mia::kCwWin - 1) / mia::kCwWin;
     const int tile_i = 32 * mia::kCwWin * es, tile_o = 32 * mia::kCwWin * eo;
@@ -605,56 +597,38 @@ bool plan_cw_bwd(const mia_ss_params &p, const DeviceInfo &di, mia::CwBwdArgs &r
     r.off_red = r.off_pf + 1024;                                // [32][20] fp32 scratch of the row reductions
     r.off_bar = r.off_red + 32 * 20 * 4;
     r.smem_bytes = r.off_bar + 8 * r.ns + 16;
-    if ((((uintptr_t)p.B | (uintptr_t)p.C) & 3) || ((p.B_batch_stride | p.B_group_stride | p.C_batch_stride | p.C_group_stride) * es) % 4) return false;
-    r.A = p.A; r.B = p.B; r.C = p.C; r.D = p.D; r.delta_bias = p.delta_bias; r.hblk = p.hblk;
-    r.B_bs = p.B_batch_stride; r.B_gs = p.B_group_stride; r.C_bs = p.C_batch_stride; r.C_gs = p.C_group_stride;
+    if (!aligned(4, {p.B, p.C}) || ((p.B_batch_stride | p.B_group_stride | p.C_batch_stride | p.C_group_stride) * es) % 4) return false;
+    r.hblk = p.hblk;
     const void *ptrs[5] = {p.u, p.delta, p.dout, p.du, p.ddelta};
     for (int i = 0; i < 5; ++i) {
         const int e = i == 2 ? eo : es;
         const int trc = mia::tma_make_2d(&tm[i], ptrs[i], trows, tcols, tcols * e, 32, mia::kCwWin, e, mia::kCwWin * e);
         if (trc != 0) { MIA_TRACE("cw bwd: tensor map %d rejected (CUresult %d)", i, trc); return false; }
     }
-    int per_sm = (227 * 1024) / (r.smem_bytes + 1024);
-    // At most 4 resident warps per SM, on the build that may use 255 registers.  On an H100 (80GB HBM3, 700 W; tools/bwd_variants.py,
-    // bf16, R = 3072) 8 warps beat 12 on the 168-register build wherever they differ - B = 16, L = 6400: 1.39 against 1.71 ms;
-    // B = 64, L = 196: 0.21 against 0.30 ms; B = 8, L = 1024: 0.136 against 0.144 ms: sm_90 issues the float2 arithmetic as two
-    // scalar instructions, so the registers buy more than the extra warps do.  Below 8 the kernel is bound by DRAM, not by issue,
-    // and fewer concurrent row streams per SM with a deeper ring move its bytes faster (same card and knobs): 4 stages at 4 warps take
-    // 0.418 ms at B = 132, L = 196 and 1.340 ms at B = 16, L = 6400, against 0.448 / 1.405 ms for 3 / 2 stages at 8 warps;
-    // 3 stages at 4 warps: 0.413 / 1.388 ms; 2 stages: 0.445 / 1.542 ms; 5-8 stages at 4 warps: 0.417 / 1.341 ms; 3 warps:
-    // >= 0.496 / 1.729 ms; 4 stages at 5-8 warps (smem allows 7): 0.429-0.461 / 1.346-1.458 ms.
-    const int cap = dbg_int("MIA_CW_MAXPERSM", 4);
-    if (per_sm > cap) per_sm = cap;
-    if (per_sm < 1) return false;
-    // at most 8 resident warps per SM: the build that may use 255 registers (scan_bwd_cw.cuh, kMinBlk); same results
-    r.wide = dbg_int("MIA_CW_WIDE", per_sm <= 8 ? 1 : 0);
-    if (r.wide && per_sm > 8) per_sm = 8;
-    const long long slots = (long long)di.sms * per_sm;
-    const long long rounds = (r.n_items + slots - 1) / slots;
-    grid = (int)((r.n_items + rounds - 1) / rounds);             // equal rounds per CTA
+    // At most 4 resident warps per SM.  The kernel is bound by DRAM, not by issue, and fewer concurrent row streams per SM with
+    // a deeper ring move its bytes faster: on an H100 (80GB HBM3, 700 W; tools/bwd_variants.py, bf16, R = 3072, debug-build knobs
+    // MIA_CW_STAGES / MIA_CW_MAXPERSM) 4 stages at 4 warps take 0.418 ms at B = 132, L = 196 and 1.340 ms at B = 16, L = 6400,
+    // against 0.448 / 1.405 ms for 3 / 2 stages at 8 warps; 3 stages at 4 warps: 0.413 / 1.388 ms; 2 stages: 0.445 / 1.542 ms;
+    // 5-8 stages at 4 warps: 0.417 / 1.341 ms; 3 warps: >= 0.496 / 1.729 ms; 4 stages at 5-8 warps (smem allows 7):
+    // 0.429-0.461 / 1.346-1.458 ms.  Never more than 8: the kernel's register budget (scan_bwd_cw.cuh).
+    const int fill = resident_grid(di, r.smem_bytes, kSmemPerSm, 1, std::min(dbg_int("MIA_CW_MAXPERSM", 4), 8), r.n_items);
+    if (!fill) return false;
+    const int rounds = (r.n_items + fill - 1) / fill;
+    grid = (r.n_items + rounds - 1) / rounds;                    // equal rounds per CTA
     return true;
 }
 
 // Deterministic d_state 16 backward (scan_bwd_rowsn.cuh): eligibility + argument block.
 bool plan_rowsn_bwd(const mia_ss_params &p, const DeviceInfo &di, mia::RowsNBwdArgs &r, int &grid) {
     const int es = esize(p.itype), eo = esize(p.otype), L = p.seqlen;
-    const int rpg = p.dim / p.n_groups;
     RowsNSplit sp;
     if (!rowsn_bwd_split(p, di.sms, kRowsNCtasPerSm, sp)) return false;
     if (dbg_knob("MIA_NO_ROWS_BWD")) return false;
-    auto dense = [&](long long bs, long long ds) { return ds == L && bs == (long long)p.dim * L; };
-    if (!dense(p.u_batch_stride, p.u_d_stride) || !dense(p.delta_batch_stride, p.delta_d_stride) ||
-        !dense(p.dout_batch_stride, p.dout_d_stride) || !dense(p.du_batch_stride, p.du_d_stride) ||
-        !dense(p.ddelta_batch_stride, p.ddelta_d_stride)) return false;
-    if (((uintptr_t)p.u | (uintptr_t)p.delta | (uintptr_t)p.dout) & 15) return false;
-    if (p.z) {
-        if (!dense(p.z_batch_stride, p.z_d_stride) || !dense(p.out_saved_batch_stride, p.out_saved_d_stride) ||
-            !dense(p.dz_batch_stride, p.dz_d_stride)) return false;
-        if (((uintptr_t)p.z | (uintptr_t)p.out_saved) & 15) return false;
-    }
-    memset(&r, 0, sizeof(r));
-    r.batch = p.batch; r.dim = p.dim; r.L = L; r.G = p.n_groups; r.rows_per_group = rpg;
-    r.softplus = p.delta_softplus; r.has_z = p.z != nullptr;
+    if (!dense_rows(p, {MIA_ROWS(u), MIA_ROWS(delta), MIA_ROWS(dout), MIA_ROWS(du), MIA_ROWS(ddelta)}) ||
+        !aligned(16, {p.u, p.delta, p.dout})) return false;
+    if (p.z && (!dense_rows(p, {MIA_ROWS(z), MIA_ROWS(out_saved), MIA_ROWS(dz)}) || !aligned(16, {p.z, p.out_saved}))) return false;
+    fill_rows_common(r, p);
+    r.has_z = p.z != nullptr;
     r.n_oct = sp.n_oct; r.oct_per_cta = sp.oct_per_cta; r.oct_per_group = sp.oct_per_group; r.max_parts = sp.max_parts;
     r.nblk = (L + mia::kRnBlk - 1) / mia::kRnBlk;
     r.Lp = r.nblk * mia::kRnBlk;
@@ -682,22 +656,27 @@ bool plan_rowsn_bwd(const mia_ss_params &p, const DeviceInfo &di, mia::RowsNBwdA
     r.off_bar = take(8);
     r.smem_bytes = off;
     if (r.smem_bytes > di.smem_optin) return false;
-    r.u = p.u; r.delta = p.delta; r.A = p.A; r.B = p.B; r.C = p.C; r.D = p.D; r.delta_bias = p.delta_bias; r.dout = p.dout;
-    r.z = p.z; r.out_saved = p.out_saved; r.du = p.du; r.ddelta = p.ddelta; r.dz = p.dz;
-    r.A_ds = p.A_d_stride; r.A_ns = p.A_dstate_stride;
-    r.B_bs = p.B_batch_stride; r.B_gs = p.B_group_stride; r.B_ns = p.B_dstate_stride;
-    r.C_bs = p.C_batch_stride; r.C_gs = p.C_group_stride; r.C_ns = p.C_dstate_stride;
+    r.dout = p.dout; r.z = p.z; r.out_saved = p.out_saved; r.du = p.du; r.ddelta = p.ddelta; r.dz = p.dz;
+    r.A_ds = p.A_d_stride; r.A_ns = p.A_dstate_stride; r.B_ns = p.B_dstate_stride; r.C_ns = p.C_dstate_stride;
     grid = sp.grid;
     return true;
 }
 
+template <typename P> using elem_t = std::remove_pointer_t<P>;
+
+// One launch for the input dtype: `f` receives a null pointer of the element type and returns the launch's error.  On success
+// counts `n_launches` kernel launches; on failure reports "<what> launch: <error>".
 template <typename F>
-int dispatch(int itype, F &&f) {
+int launch(int itype, const char *what, int n_launches, F &&f) {
+    cudaError_t e;
     switch (itype) {
-        case MIA_F32: return f((float *)nullptr);
-        case MIA_F16: return f((__half *)nullptr);
-        default: return f((__nv_bfloat16 *)nullptr);
+        case MIA_F32: e = f((float *)nullptr); break;
+        case MIA_F16: e = f((__half *)nullptr); break;
+        default: e = f((__nv_bfloat16 *)nullptr); break;
     }
+    if (e != cudaSuccess) return fail(MIA_ECUDA, "%s launch: %s", what, cudaGetErrorString(e));
+    g_launches.fetch_add(n_launches);
+    return MIA_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -831,91 +810,50 @@ int mia_selective_scan_fwd(const mia_ss_params *pp, void *cuda_stream) {
     DeviceInfo di;
     if (int rc = device_info(di)) return rc;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
+    const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
+    int grid = 0;
+    // The first family that takes the problem runs: column-walk, chunk-parallel, resident-row, streaming, d_state 8 / 16
+    // row-serial, warp-scan.
     {
         mia::CwFwdArgs r;
         CUtensorMap tm[3];
-        int rgrid = 0;
-        if (plan_cw_fwd(p, di, r, tm, rgrid)) {
-            MIA_TRACE("fwd: cw g=%d ns=%d nwin=%d grid=%d smem=%d", r.g, r.ns, r.nwin, rgrid, r.smem_bytes);
-            const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
-            const int rc = dispatch(p.itype, [&](auto *tag) {
-                using T = typename std::remove_pointer<decltype(tag)>::type;
-                return (int)mia::launch_fwd_cw<T>(tm, r, rgrid, of32, stream);
-            });
-            if (rc != 0) return fail(MIA_ECUDA, "selective_scan_fwd (column-walk) launch: %s", cudaGetErrorString((cudaError_t)rc));
-            g_launches.fetch_add(1);
-            return MIA_OK;
+        if (plan_cw_fwd(p, di, r, tm, grid)) {
+            MIA_TRACE("fwd: cw g=%d ns=%d nwin=%d grid=%d smem=%d", r.g, r.ns, r.nwin, grid, r.smem_bytes);
+            return launch(p.itype, "selective_scan_fwd (column-walk)", 1,
+                          [&](auto *t) { return mia::launch_fwd_cw<elem_t<decltype(t)>>(tm, r, grid, of32, stream); });
         }
     }
     {
         mia::ChunkArgs r;
-        int rgrid = 0;
-        if (plan_chunks_fwd(p, di, r, rgrid)) {
-            const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
-            const int rc = dispatch(p.itype, [&](auto *tag) {
-                using T = typename std::remove_pointer<decltype(tag)>::type;
-                return (int)mia::launch_fwd_chunks<T>(r, rgrid, of32, stream);
-            });
-            if (rc != 0) return fail(MIA_ECUDA, "selective_scan_fwd (chunk-parallel) launch: %s", cudaGetErrorString((cudaError_t)rc));
-            g_launches.fetch_add(3);
-            return MIA_OK;
-        }
+        if (plan_chunks_fwd(p, di, r, grid))
+            return launch(p.itype, "selective_scan_fwd (chunk-parallel)", 3,
+                          [&](auto *t) { return mia::launch_fwd_chunks<elem_t<decltype(t)>>(r, grid, of32, stream); });
     }
     {
         mia::RowsArgs r;
-        int rgrid = 0;
-        if (plan_rows_fwd(p, di, r, rgrid)) {
-            const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
-            const int rc = dispatch(p.itype, [&](auto *tag) {
-                using T = typename std::remove_pointer<decltype(tag)>::type;
-                return (int)mia::launch_fwd_rows<T>(r, rgrid, of32, stream);
-            });
-            if (rc != 0) return fail(MIA_ECUDA, "selective_scan_fwd (row-serial) launch: %s", cudaGetErrorString((cudaError_t)rc));
-            g_launches.fetch_add(1);
-            return MIA_OK;
-        }
+        if (plan_rows_fwd(p, di, r, grid))
+            return launch(p.itype, "selective_scan_fwd (row-serial)", 1,
+                          [&](auto *t) { return mia::launch_fwd_rows<elem_t<decltype(t)>>(r, grid, of32, stream); });
     }
     {
         mia::StreamArgs r;
-        int rgrid = 0;
-        if (plan_stream_fwd(p, di, r, rgrid)) {
-            const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
-            const int rc = dispatch(p.itype, [&](auto *tag) {
-                using T = typename std::remove_pointer<decltype(tag)>::type;
-                return (int)mia::launch_fwd_stream<T>(r, rgrid, of32, stream);
-            });
-            if (rc != 0) return fail(MIA_ECUDA, "selective_scan_fwd (streaming) launch: %s", cudaGetErrorString((cudaError_t)rc));
-            g_launches.fetch_add(1);
-            return MIA_OK;
-        }
+        if (plan_stream_fwd(p, di, r, grid))
+            return launch(p.itype, "selective_scan_fwd (streaming)", 1,
+                          [&](auto *t) { return mia::launch_fwd_stream<elem_t<decltype(t)>>(r, grid, of32, stream); });
     }
     {
         mia::RowsNArgs r;
-        int rgrid = 0;
-        if (plan_rowsn_fwd(p, di, r, rgrid)) {
-            const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
-            const int rc = dispatch(p.itype, [&](auto *tag) {
-                using T = typename std::remove_pointer<decltype(tag)>::type;
-                return (int)mia::launch_fwd_rowsn<T>(r, rgrid, of32, stream);
-            });
-            if (rc != 0) return fail(MIA_ECUDA, "selective_scan_fwd (row-serial, d_state %d) launch: %s", p.dstate, cudaGetErrorString((cudaError_t)rc));
-            g_launches.fetch_add(1);
-            return MIA_OK;
-        }
+        if (plan_rowsn_fwd(p, di, r, grid))
+            return launch(p.itype, "selective_scan_fwd (row-serial, d_state 8 / 16)", 1,
+                          [&](auto *t) { return mia::launch_fwd_rowsn<elem_t<decltype(t)>>(r, grid, of32, stream); });
     }
     Plan pl;
     mia::ScanArgs a;
     if (int rc = plan_and_layout(p, di, false, pl, a)) return rc;
     a.out = p.out; a.out_z = p.out_z;
     a.out_bs = p.out_batch_stride; a.out_ds = p.out_d_stride; a.outz_bs = p.out_z_batch_stride; a.outz_ds = p.out_z_d_stride;
-    const int grid = a.n_seg < di.sms ? a.n_seg : di.sms;
-    const int rc = dispatch(p.itype, [&](auto *tag) {
-        using T = typename std::remove_pointer<decltype(tag)>::type;
-        return (int)mia::launch_fwd_any<T>(a, grid, stream);
-    });
-    if (rc != 0) return fail(MIA_ECUDA, "selective_scan_fwd launch: %s", cudaGetErrorString((cudaError_t)rc));
-    g_launches.fetch_add(1);
-    return MIA_OK;
+    grid = a.n_seg < di.sms ? a.n_seg : di.sms;
+    return launch(p.itype, "selective_scan_fwd", 1, [&](auto *t) { return mia::launch_fwd_any<elem_t<decltype(t)>>(a, grid, stream); });
 }
 
 }  // extern "C"
@@ -974,71 +912,52 @@ int bwd_impl(const mia_ss_params *pp, void *cuda_stream, bool det) {
     a.ddelta_full = (float *)(ws + w.ddelta_full);
     a.bc_atomic = w.bc_atomic;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
+    const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
+    auto give_partials = [&](auto &r) {
+        r.part_dA = a.part_dA; r.part_dD = a.part_dD; r.part_dbias = a.part_dbias; r.acc_dB = a.acc_dB; r.acc_dC = a.acc_dC;
+    };
+    // The first family that takes the problem runs: d_state 16 row-serial, column-walk, resident-row, (deterministic)
+    // warp-scan.  Then the finalize kernel folds the partials.
     mia::RowsNBwdArgs rn;
-    int rn_grid = 0;
-    const bool use_rowsn = plan_rowsn_bwd(p, di, rn, rn_grid);
-    if (use_rowsn) a.bc_atomic = 0;
-    if (a.bc_atomic) {
-        MIA_CUDA(cudaMemsetAsync(a.acc_dB, 0, w.acc_bytes, stream));
-        MIA_CUDA(cudaMemsetAsync(a.acc_dC, 0, w.acc_bytes, stream));
-        g_launches.fetch_add(2);
-    }
-    int rc = 0, bc_parts = pl.split;
-    mia::RowsBwdArgs rb;
-    int rgrid = 0;
-    CUtensorMap tmaps[5];
-    // Column-walk kernel (one warp per 32 g rows, phase 2 only, on the forward's block states): short rows always; rows of more
-    // than one 256-token chunk only with enough 32-row items to fill the SMs (four per SM); below that a
-    // one-warp-per-item walk leaves the SMs short of warps and the warp-scan kernel is used.
-    const long long items32 = (long long)p.batch * (p.dim / 32);
     mia::CwBwdArgs cwb;
-    const bool want_cw = !use_rowsn && p.hblk && (p.seqlen <= mia::kRowsChunk || items32 >= 4LL * di.sms || dbg_knob("MIA_FORCE_CW_BWD"));
-    if (want_cw && plan_cw_bwd(p, di, cwb, tmaps, rgrid)) {
-        MIA_TRACE("bwd: cw g=%d ns=%d ngrp=%d grid=%d smem=%d", cwb.g, cwb.ns, cwb.ngrp, rgrid, cwb.smem_bytes);
-        cwb.part_dA = a.part_dA; cwb.part_dD = a.part_dD; cwb.part_dbias = a.part_dbias; cwb.acc_dB = a.acc_dB; cwb.acc_dC = a.acc_dC;
-        bc_parts = cwb.rows_per_group / 32;
-        const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
-        rc = dispatch(p.itype, [&](auto *tag) {
-            using T = typename std::remove_pointer<decltype(tag)>::type;
-            return (int)mia::launch_bwd_cw<T>(tmaps, cwb, rgrid, of32, stream);
-        });
-    } else if (use_rowsn) {
-        rn.part_dA = a.part_dA; rn.part_dD = a.part_dD; rn.part_dbias = a.part_dbias; rn.acc_dB = a.acc_dB; rn.acc_dC = a.acc_dC;
+    mia::RowsBwdArgs rb;
+    CUtensorMap tmaps[5];
+    int rc, grid = 0, bc_parts = pl.split;
+    const bool use_rowsn = plan_rowsn_bwd(p, di, rn, grid);
+    if (use_rowsn) {
+        a.bc_atomic = 0;
+        give_partials(rn);
         bc_parts = rn.max_parts;
-        const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
-        rc = dispatch(p.itype, [&](auto *tag) {
-            using T = typename std::remove_pointer<decltype(tag)>::type;
-            return (int)mia::launch_bwd_rowsn<T>(rn, rn_grid, of32, stream);
-        });
-    } else if (plan_rows_bwd(p, di, rb, rgrid)) {
-        rb.part_dA = a.part_dA; rb.part_dD = a.part_dD; rb.part_dbias = a.part_dbias; rb.acc_dB = a.acc_dB; rb.acc_dC = a.acc_dC;
+        rc = launch(p.itype, "selective_scan_bwd", 1, [&](auto *t) { return mia::launch_bwd_rowsn<elem_t<decltype(t)>>(rn, grid, of32, stream); });
+    } else if (plan_cw_bwd(p, di, cwb, tmaps, grid)) {
+        MIA_TRACE("bwd: cw g=%d ns=%d ngrp=%d grid=%d smem=%d", cwb.g, cwb.ns, cwb.ngrp, grid, cwb.smem_bytes);
+        give_partials(cwb);
+        bc_parts = cwb.rows_per_group / 32;
+        rc = launch(p.itype, "selective_scan_bwd", 1, [&](auto *t) { return mia::launch_bwd_cw<elem_t<decltype(t)>>(tmaps, cwb, grid, of32, stream); });
+    } else if (plan_rows_bwd(p, di, rb, grid)) {
+        give_partials(rb);
         bc_parts = rb.rows_per_group / 32;
-        const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
-        rc = dispatch(p.itype, [&](auto *tag) {
-            using T = typename std::remove_pointer<decltype(tag)>::type;
-            return (int)mia::launch_bwd_rows<T>(rb, rgrid, of32, stream);
-        });
-    } else if (det) {
-        const int grid = a.n_seg < di.sms ? a.n_seg : di.sms;
-#ifdef MIA_DEBUG
-        a.det_status = det_status_word();
-        if (a.det_status) MIA_CUDA(cudaMemsetAsync(a.det_status, 0, sizeof(int), stream));
-#endif
-        MIA_TRACE("bwd: deterministic warp-scan N=%d LPR=%d split=%d n_seg=%d RT=%d stages=%d smem=%d smem_acc=%d grid=%d", p.dstate,
-                  a.LPR, a.split, a.n_seg, a.RT, a.stages, a.smem_bytes, a.det_smem_acc, grid);
-        rc = dispatch(p.itype, [&](auto *tag) {
-            using T = typename std::remove_pointer<decltype(tag)>::type;
-            return (int)mia::launch_bwd_det<T>(a, grid, stream);
-        });
+        rc = launch(p.itype, "selective_scan_bwd", 1, [&](auto *t) { return mia::launch_bwd_rows<elem_t<decltype(t)>>(rb, grid, of32, stream); });
     } else {
-        const int grid = a.n_seg < di.sms ? a.n_seg : di.sms;
-        rc = dispatch(p.itype, [&](auto *tag) {
-            using T = typename std::remove_pointer<decltype(tag)>::type;
-            return (int)mia::launch_bwd_any<T>(a, grid, stream);
-        });
+        if (a.bc_atomic) {
+            MIA_CUDA(cudaMemsetAsync(a.acc_dB, 0, w.acc_bytes, stream));
+            MIA_CUDA(cudaMemsetAsync(a.acc_dC, 0, w.acc_bytes, stream));
+            g_launches.fetch_add(2);
+        }
+        grid = a.n_seg < di.sms ? a.n_seg : di.sms;
+        if (det) {
+#ifdef MIA_DEBUG
+            a.det_status = det_status_word();
+            if (a.det_status) MIA_CUDA(cudaMemsetAsync(a.det_status, 0, sizeof(int), stream));
+#endif
+            MIA_TRACE("bwd: deterministic warp-scan N=%d LPR=%d split=%d n_seg=%d RT=%d stages=%d smem=%d smem_acc=%d grid=%d", p.dstate,
+                      a.LPR, a.split, a.n_seg, a.RT, a.stages, a.smem_bytes, a.det_smem_acc, grid);
+            rc = launch(p.itype, "selective_scan_bwd", 1, [&](auto *t) { return mia::launch_bwd_det<elem_t<decltype(t)>>(a, grid, stream); });
+        } else {
+            rc = launch(p.itype, "selective_scan_bwd", 1, [&](auto *t) { return mia::launch_bwd_any<elem_t<decltype(t)>>(a, grid, stream); });
+        }
     }
-    if (rc != 0) return fail(MIA_ECUDA, "selective_scan_bwd launch: %s", cudaGetErrorString((cudaError_t)rc));
-    g_launches.fetch_add(1);
+    if (rc) return rc;
 
     FinArgs f;
     memset(&f, 0, sizeof(f));
@@ -1060,13 +979,11 @@ int bwd_impl(const mia_ss_params *pp, void *cuda_stream, bool det) {
     const long long total = (2 * f.n_bc + f.n_dd + 31) / 32 * 32 + 32 * (f.n_dA + f.n_dD + f.n_db);
     long long blocks = (total + 255) / 256;
     if (blocks > di.sms * 8) blocks = di.sms * 8;
-    rc = dispatch(p.itype, [&](auto *tag) {
-        using T = typename std::remove_pointer<decltype(tag)>::type;
-        ss_finalize_kernel<T><<<(int)blocks, 256, 0, stream>>>(f);
-        return (int)cudaGetLastError();
+    rc = launch(p.itype, "selective_scan_bwd finalize", 1, [&](auto *t) {
+        ss_finalize_kernel<elem_t<decltype(t)>><<<(int)blocks, 256, 0, stream>>>(f);
+        return cudaGetLastError();
     });
-    if (rc != 0) return fail(MIA_ECUDA, "selective_scan_bwd finalize launch: %s", cudaGetErrorString((cudaError_t)rc));
-    g_launches.fetch_add(1);
+    if (rc) return rc;
 #ifdef MIA_DEBUG
     if (a.det_status) {
         int st = 0;

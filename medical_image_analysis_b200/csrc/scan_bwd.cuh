@@ -488,10 +488,7 @@ cudaError_t launch_bwd(const ScanArgs &a, int grid, cudaStream_t stream) {
         else kernel = n1 ? MIA_PICK(false, true) : MIA_PICK(false, false);
     }
 #undef MIA_PICK
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, kThreads, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, kThreads, a.smem_bytes, stream, a);
 }
 
 }  // namespace mia

@@ -30,9 +30,6 @@
 
 namespace mia {
 
-#ifndef MIA_CW_FMA
-#define MIA_CW_FMA 0             // 1: h_t by one FFMA (a_t h_{t-1} off the serial chain); compare with tools/ab_cw.py
-#endif
 constexpr int kCwGrp = 16;       // columns per group = tokens per recompute block
 constexpr int kCwWin = 32;       // columns per window = per stage of the ring (two groups)
 
@@ -40,7 +37,7 @@ struct CwBwdArgs {
     int batch, dim, L, G, rows_per_group;
     int softplus;
     int g, n_items, ngrp, nwin, ns;         // rows per tensor-map row; items of 32 g rows; 16-column groups / 32-column windows per tensor-map row; stages
-    int wide;                               // at most 8 resident warps per SM planned: the build with up to 255 registers per thread
+    int unused;                             // 0, kept so that the kernel's code stays as measured
     int stage_bytes, off_bc32, off_pf, off_red, off_bar, smem_bytes;
     const void *A, *B, *C, *D, *delta_bias;
     const float *hblk;
@@ -95,7 +92,7 @@ __device__ __forceinline__ void cw_bwd_block(const int qlo_in, const int qhi_in,
     float h = h0;
     // Tile accesses: one quad (4 tokens) at a time, or -- whole blocks of 2-byte types -- two quads = ONE 16-byte access per tile
     // and lane, which is conflict-free on the swizzled tile where the 8-byte accesses are not (Oct, scan_fwd_rows.cuh).
-    constexpr bool kOct = kFull && es == 2 && MIA_CW_OCT;
+    constexpr bool kOct = kFull && es == 2;
     constexpr int kNQ = kOct ? 2 : 1, kNP = 2 * kNQ, kNS = 4 / kNQ;
     auto ld_in = [&](const char *tile, const int q0, float2(&f)[kNP]) {
         if constexpr (kOct) Oct<T>::ld(tile + ri.at(wbi + 4 * q0 * es), f);
@@ -134,13 +131,8 @@ __device__ __forceinline__ void cw_bwd_block(const int qlo_in, const int qhi_in,
                 const float2 bv = mul2(mul2(m, uu[p]), Bv[p]);
                 float2 hp, hh;
                 // a_t h_{t-1}, then h_t
-#if MIA_CW_FMA
-                hp.x = __fmul_rn(av.x, h); h = fmaf(av.x, h, bv.x); hh.x = h;
-                hp.y = __fmul_rn(av.y, h); h = fmaf(av.y, h, bv.y); hh.y = h;
-#else
                 hp.x = av.x * h; h = hp.x + bv.x; hh.x = h;
                 hp.y = av.y * h; h = hp.y + bv.y; hh.y = h;
-#endif
                 R.a[k] = av; R.hp[k] = hp; R.m[k] = m;
                 const float2 dCv = mul2(dy[p], hh);
                 v[2 * k] = dCv.x; v[2 * k + 1] = dCv.y;
@@ -193,13 +185,13 @@ __device__ __forceinline__ void cw_bwd_block(const int qlo_in, const int qhi_in,
     if (mine && lane < 16) accB[tok0 + i16] = dBt * kLn2;
 }
 
-// kMinBlk = resident one-warp CTAs per SM the register allocation is sized for: 12 -> 168 registers (three warps per scheduler);
-// 8 -> ptxas takes 247 and has no spills: same instructions, scheduled with the loads hoisted further.  The planner runs at
-// most 4 warps per SM (plan_cw_bwd), so that build costs no residency.
-template <typename T, bool kSoftplus, bool kOutF32, int kG, int kMinBlk>
-__global__ void __launch_bounds__(32, kMinBlk) ss_bwd_cw_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_d,
-                                                           const __grid_constant__ CUtensorMap tm_o, const __grid_constant__ CUtensorMap tm_du,
-                                                           const __grid_constant__ CUtensorMap tm_dd, const __grid_constant__ CwBwdArgs a) {
+// Register allocation sized for 8 resident one-warp CTAs per SM: ptxas takes up to 255 registers and spills nothing.  A
+// 12-warp (168-register) build ran slower wherever the two differed (DESIGN.md 3.7), and the planner keeps at most 4 warps
+// per SM resident (plan_cw_bwd), so this budget costs no residency.
+template <typename T, bool kSoftplus, bool kOutF32, int kG>
+__global__ void __launch_bounds__(32, 8) ss_bwd_cw_kernel(const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_d,
+                                                     const __grid_constant__ CUtensorMap tm_o, const __grid_constant__ CUtensorMap tm_du,
+                                                     const __grid_constant__ CUtensorMap tm_dd, const __grid_constant__ CwBwdArgs a) {
     // The swizzled tiles need 1024-byte alignment.  The dynamic shared memory of a kernel without static shared memory starts at
     // the CTA's shared window, which is allocated in 1 KB units: asserted once instead of re-aligned at run time (the re-alignment
     // cost a register and ~10 instructions per step).
@@ -415,20 +407,12 @@ __global__ void __launch_bounds__(32, kMinBlk) ss_bwd_cw_kernel(const __grid_con
     if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
-template <typename T, int kG, int kMinBlk>
-cudaError_t launch_bwd_cw_gm(const CUtensorMap *tm, const CwBwdArgs &a, int grid, bool dout_f32, cudaStream_t stream) {
-    void (*kernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CwBwdArgs);
-    if (a.softplus) kernel = dout_f32 ? &ss_bwd_cw_kernel<T, true, true, kG, kMinBlk> : &ss_bwd_cw_kernel<T, true, false, kG, kMinBlk>;
-    else kernel = dout_f32 ? &ss_bwd_cw_kernel<T, false, true, kG, kMinBlk> : &ss_bwd_cw_kernel<T, false, false, kG, kMinBlk>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, 32, a.smem_bytes, stream>>>(tm[0], tm[1], tm[2], tm[3], tm[4], a);
-    return cudaGetLastError();
-}
-
 template <typename T, int kG>
 cudaError_t launch_bwd_cw_g(const CUtensorMap *tm, const CwBwdArgs &a, int grid, bool dout_f32, cudaStream_t stream) {
-    return a.wide ? launch_bwd_cw_gm<T, kG, 8>(tm, a, grid, dout_f32, stream) : launch_bwd_cw_gm<T, kG, 12>(tm, a, grid, dout_f32, stream);
+    void (*kernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CwBwdArgs);
+    if (a.softplus) kernel = dout_f32 ? &ss_bwd_cw_kernel<T, true, true, kG> : &ss_bwd_cw_kernel<T, true, false, kG>;
+    else kernel = dout_f32 ? &ss_bwd_cw_kernel<T, false, true, kG> : &ss_bwd_cw_kernel<T, false, false, kG>;
+    return launch_smem(kernel, grid, 32, a.smem_bytes, stream, tm[0], tm[1], tm[2], tm[3], tm[4], a);
 }
 
 template <typename T>

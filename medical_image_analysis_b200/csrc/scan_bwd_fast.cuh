@@ -241,10 +241,7 @@ cudaError_t launch_bwd_any(const ScanArgs &a, int grid, cudaStream_t stream) {
         if (a.softplus) kernel = of32 ? &ss_bwd_fastn_kernel<T, true, true> : &ss_bwd_fastn_kernel<T, true, false>;
         else kernel = of32 ? &ss_bwd_fastn_kernel<T, false, true> : &ss_bwd_fastn_kernel<T, false, false>;
     }
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, kThreads, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, kThreads, a.smem_bytes, stream, a);
 }
 
 // The deterministic d_state > 1 backward: the same kernel choice as launch_bwd_any, kDet instantiations
@@ -258,10 +255,7 @@ cudaError_t launch_bwd_det(const ScanArgs &a, int grid, cudaStream_t stream) {
     const bool of32 = a.out_f32 || sizeof(T) == 4;
     if (a.softplus) kernel = of32 ? &ss_bwd_fastn_kernel<T, true, true, true> : &ss_bwd_fastn_kernel<T, true, false, true>;
     else kernel = of32 ? &ss_bwd_fastn_kernel<T, false, true, true> : &ss_bwd_fastn_kernel<T, false, false, true>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, kThreads, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, kThreads, a.smem_bytes, stream, a);
 }
 
 }  // namespace mia

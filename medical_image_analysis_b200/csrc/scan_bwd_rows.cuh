@@ -369,10 +369,7 @@ cudaError_t launch_bwd_rows(const RowsBwdArgs &a, int grid, bool dout_f32, cudaS
     void (*kernel)(const RowsBwdArgs);
     if (a.softplus) kernel = dout_f32 ? &ss_bwd_rows_kernel<T, true, true> : &ss_bwd_rows_kernel<T, true, false>;
     else kernel = dout_f32 ? &ss_bwd_rows_kernel<T, false, true> : &ss_bwd_rows_kernel<T, false, false>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, 64, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, 64, a.smem_bytes, stream, a);
 }
 
 }  // namespace mia

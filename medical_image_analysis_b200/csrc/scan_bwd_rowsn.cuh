@@ -422,10 +422,7 @@ cudaError_t launch_bwd_rowsn(const RowsNBwdArgs &a, int grid, bool dout_f32, cud
     if (sp) kernel = hz ? MIA_PICK(true, true) : MIA_PICK(true, false);
     else kernel = hz ? MIA_PICK(false, true) : MIA_PICK(false, false);
 #undef MIA_PICK
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, 32 * kRnWarps, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, 32 * kRnWarps, a.smem_bytes, stream, a);
 }
 
 }  // namespace mia

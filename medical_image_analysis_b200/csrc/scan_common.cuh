@@ -40,8 +40,8 @@ struct ScanArgs {
     int row_pitch, rowo_pitch, bc_pitch;
     int off_u, off_delta, off_z, off_dout, off_osaved, off_h0, stage_bytes;   // inside a row stage
     int goff_B, goff_C, goff_A, goff_D, goff_bias, gstage_bytes;              // inside a group stage
-    int off_groups, off_bars, off_carry, off_red, off_bcf, smem_bytes;        // row stages start at 0; off_bcf: fp32 B/C chunk
-                                                                              // of the d_state > 1 fast backward (0 = absent)
+    int off_groups, off_bars, off_carry, off_red, unused, smem_bytes;         // row stages start at 0; unused: 0, kept so
+                                                                              // that the kernels' code stays as measured
     // pointers
     const void *u, *delta, *A, *B, *C, *D, *delta_bias, *z;
     void *out, *out_z;
@@ -63,6 +63,15 @@ struct ScanArgs {
     int off_det, off_det_acc, det_smem_acc;
     int *det_status;
 };
+
+// Host: opt `kernel` in to `smem` bytes of dynamic shared memory, launch it, and return the first error.
+template <typename... P, typename... A>
+cudaError_t launch_smem(void (*kernel)(P...), int grid, int block, int smem, cudaStream_t stream, const A &...args) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return e;
+    kernel<<<grid, block, smem, stream>>>(args...);
+    return cudaGetLastError();
+}
 
 // ------------------------------------------------------------------------------------------------
 // PTX wrappers: mbarrier, TMA bulk copy, fast math.

@@ -248,10 +248,7 @@ cudaError_t launch_fwd(const ScanArgs &a, int grid, cudaStream_t stream) {
     if (a.softplus) kernel = n1 ? MIA_PICK(true, true) : MIA_PICK(true, false);
     else kernel = n1 ? MIA_PICK(false, true) : MIA_PICK(false, false);
 #undef MIA_PICK
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, kThreadsFwd, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, kThreadsFwd, a.smem_bytes, stream, a);
 }
 
 }  // namespace mia

@@ -158,15 +158,12 @@ cudaError_t launch_fwd_chunks(const ChunkArgs &a, int grid, bool out_f32, cudaSt
     void (*kc)(const ChunkArgs);
     if (a.softplus) kc = out_f32 ? &ss_fwd_chunk_kernel<T, true, true, false> : &ss_fwd_chunk_kernel<T, true, false, false>;
     else kc = out_f32 ? &ss_fwd_chunk_kernel<T, false, true, false> : &ss_fwd_chunk_kernel<T, false, false, false>;
-    cudaError_t e = cudaFuncSetAttribute(ka, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
+    const cudaError_t e = cudaFuncSetAttribute(ka, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
     if (e != cudaSuccess) return e;
     ka<<<grid, 32, a.smem_bytes, stream>>>(a);
     const int n_rows = a.batch * a.dim;
     ss_fwd_chunk_combine_kernel<T><<<(n_rows + 255) / 256, 256, 0, stream>>>(reinterpret_cast<float2 *>(a.x), n_rows, a.n_chunks);
-    kc<<<grid, 32, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kc, grid, 32, a.smem_bytes, stream, a);
 }
 
 }  // namespace mia

@@ -36,9 +36,6 @@
 namespace mia {
 
 constexpr int kCwTok = 32;       // columns per window
-#ifndef MIA_CW_OCT
-#define MIA_CW_OCT 1             // 0: the 8-byte (quad) tile accesses of the first version, kept for A/B timing (tools/ab_cw.py)
-#endif
 
 struct CwFwdArgs {
     int batch, dim, L, G, rows_per_group;
@@ -92,7 +89,7 @@ __global__ void __launch_bounds__(32, 16) ss_fwd_cw_kernel(const __grid_constant
     using raw = typename Cvt<T>::raw;
     constexpr int RBi = kCwTok * es, RBo = kCwTok * eo;
     constexpr int kTileI = 32 * RBi, kTileO = 32 * RBo;
-    constexpr bool kOct = es == 2 && MIA_CW_OCT;                         // 16-byte tile accesses (8 tokens) for 2-byte types
+    constexpr bool kOct = es == 2;                                       // 16-byte tile accesses (8 tokens) for 2-byte types
     const int lane = threadIdx.x;
     float *Bw = reinterpret_cast<float *>(smem + a.off_bc32), *Cw = Bw + kCwTok;
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + a.off_bar);
@@ -319,10 +316,7 @@ cudaError_t launch_fwd_cw_g(const CUtensorMap *tm, const CwFwdArgs &a, int grid,
     void (*kernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CwFwdArgs);
     if (a.softplus) kernel = out_f32 ? &ss_fwd_cw_kernel<T, true, true, kG> : &ss_fwd_cw_kernel<T, true, false, kG>;
     else kernel = out_f32 ? &ss_fwd_cw_kernel<T, false, true, kG> : &ss_fwd_cw_kernel<T, false, false, kG>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, 32, a.smem_bytes, stream>>>(tm[0], tm[1], tm[2], a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, 32, a.smem_bytes, stream, tm[0], tm[1], tm[2], a);
 }
 
 template <typename T>

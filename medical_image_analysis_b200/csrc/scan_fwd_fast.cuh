@@ -159,10 +159,7 @@ cudaError_t launch_fwd_any(const ScanArgs &a, int grid, cudaStream_t stream) {
     const bool of32 = a.out_f32 || sizeof(T) == 4;
     if (a.softplus) kernel = of32 ? &ss_fwd_fast_kernel<T, true, true> : &ss_fwd_fast_kernel<T, true, false>;
     else kernel = of32 ? &ss_fwd_fast_kernel<T, false, true> : &ss_fwd_fast_kernel<T, false, false>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, kThreadsFwd, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, kThreadsFwd, a.smem_bytes, stream, a);
 }
 
 }  // namespace mia

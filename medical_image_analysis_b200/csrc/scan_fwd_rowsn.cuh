@@ -271,10 +271,7 @@ cudaError_t launch_fwd_rowsn(const RowsNArgs &a, int grid, bool out_f32, cudaStr
     if (a.N == 16) kernel = hz ? pick_fwd_rowsn<T, 16, true>(sp, out_f32) : pick_fwd_rowsn<T, 16, false>(sp, out_f32);
     else if (a.N == 8) kernel = hz ? pick_fwd_rowsn<T, 8, true>(sp, out_f32) : pick_fwd_rowsn<T, 8, false>(sp, out_f32);
     else return cudaErrorInvalidValue;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, 32 * a.warps, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, 32 * a.warps, a.smem_bytes, stream, a);
 }
 
 }  // namespace mia

@@ -180,10 +180,7 @@ cudaError_t launch_fwd_stream(const StreamArgs &a, int grid, bool out_f32, cudaS
     void (*kernel)(const StreamArgs);
     if (a.softplus) kernel = out_f32 ? &ss_fwd_stream_kernel<T, true, true> : &ss_fwd_stream_kernel<T, true, false>;
     else kernel = out_f32 ? &ss_fwd_stream_kernel<T, false, true> : &ss_fwd_stream_kernel<T, false, false>;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, 32, a.smem_bytes, stream>>>(a);
-    return cudaGetLastError();
+    return launch_smem(kernel, grid, 32, a.smem_bytes, stream, a);
 }
 
 }  // namespace mia

@@ -33,8 +33,7 @@ VARIANTS = {
     "no_hblk": None,          # backward without block states: resident-row / warp-scan kernels
 }
 for _ns in (2, 3):
-    for _cap in (8, 12):
-        VARIANTS[f"cw_ns{_ns}_cap{_cap}"] = {"MIA_FORCE_CW_BWD": "1", "MIA_CW_STAGES": str(_ns), "MIA_CW_MAXPERSM": str(_cap)}
+    VARIANTS[f"cw_ns{_ns}_cap8"] = {"MIA_FORCE_CW_BWD": "1", "MIA_CW_STAGES": str(_ns), "MIA_CW_MAXPERSM": "8"}
 
 
 def main():
