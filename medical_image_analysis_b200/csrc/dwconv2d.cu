@@ -114,15 +114,28 @@ __device__ __forceinline__ void store_planes(typename mia::Cvt<T>::raw *g, size_
     }
 }
 
+// The forward's dynamic shared memory, offsets in floats from its base: sx [P][(H + 2) (W + 2)], taps [P][12] (10 used),
+// so [P][HW] staged results in the tensor's dtype.  sx is rounded up to 4 floats so that taps and so start on 16-byte
+// boundaries for every shape: the vector path copies so out as uint4.
+struct DwFwdSmem {
+    int taps, so;
+    size_t bytes;
+};
+__host__ __device__ __forceinline__ DwFwdSmem dw_fwd_smem(int P, int H, int W, int es) {
+    const int sx = (P * (H + 2) * (W + 2) + 3) & ~3;
+    return {sx, sx + P * 12, (size_t)(sx + P * 12) * sizeof(float) + (size_t)P * H * W * es};
+}
+
 // ------------------------------------------------------------------------------------------------ forward
 template <typename T, bool kSilu, int kV>
 __global__ void __launch_bounds__(kDwThreads) dwconv2d_fwd_kernel(const DwArgs a) {
     using raw = typename mia::Cvt<T>::raw;
     extern __shared__ __align__(16) char dsm[];
     const int H = a.H, W = a.W, HW = H * W, Wp = W + 2, PS = (H + 2) * Wp, P = a.planes_per_block;
-    float *sx = reinterpret_cast<float *>(dsm);               // [P][(H + 2) (W + 2)]
-    float *taps = sx + (size_t)P * PS;                        // [P][10] (padded to 12)
-    raw *so = reinterpret_cast<raw *>(taps + (size_t)P * 12); // [P][HW] staged results
+    const DwFwdSmem lay = dw_fwd_smem(P, H, W, (int)sizeof(raw));
+    float *sx = reinterpret_cast<float *>(dsm);
+    float *taps = sx + lay.taps;
+    raw *so = reinterpret_cast<raw *>(sx + lay.so);
     const int n_planes = a.batch * a.C;
     zero_planes(sx, P * PS);                                  // the borders stay zero for the whole kernel
     __syncthreads();
@@ -243,11 +256,28 @@ __global__ void __launch_bounds__(kDwThreads) dwconv2d_bwd_kernel(const DwArgs a
 thread_local char g_dw_err[256] = "";
 uint32_t dw_magic(int d) { return d == 1 ? 0u : (uint32_t)((0x100000000ULL + (uint64_t)d - 1) / (uint64_t)d); }
 
-int dw_check(const void *x, int batch, int C, int H, int W, int dtype) {
+constexpr size_t kDwSmemMax = 227 * 1024;   // sm_90's opt-in limit of dynamic shared memory per block
+
+size_t dw_bwd_smem(int P, int H, int W, int es) { return (size_t)2 * P * (H + 2) * (W + 2) * sizeof(float) + (size_t)P * H * W * es; }
+
+// Validates the call and sizes its blocks: P planes per block (forward: staged per pass, at most 16; backward: batch planes
+// per pass) and the dynamic shared memory they take.  Thin planes do not fit (a 1 x 16384 fp32 forward, a 4 x 4096 fp32
+// backward): they are rejected here, before any CUDA call.
+int dw_check(const void *x, int batch, int C, int H, int W, int dtype, bool bwd, int &P, size_t &smem) {
     if (!x || batch <= 0 || C <= 0 || H <= 0 || W <= 0) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d: empty or null input"); return MIA_EINVAL; }
     if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d: bad dtype"); return MIA_EINVAL; }
     if ((long long)H * W > 16384) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d: planes larger than 16384 elements are not supported"); return MIA_EINVAL; }
     if ((long long)batch * C >= (1LL << 31) / 2) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d: batch*channels too large"); return MIA_EINVAL; }
+    const int es = dtype == MIA_F32 ? 4 : 2;
+    P = 2048 / (H * W);
+    if (P < 1) P = 1;
+    if (P > (bwd ? batch : 16)) P = bwd ? batch : 16;
+    smem = bwd ? dw_bwd_smem(P, H, W, es) : dw_fwd_smem(P, H, W, es).bytes;
+    if (smem > kDwSmemMax) {
+        snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d_%s: a %d x %d %s plane needs %zu bytes of shared memory per block, more than the "
+                 "%zu-byte (227 KB) limit", bwd ? "bwd" : "fwd", H, W, es == 4 ? "float32" : "16-bit", smem, kDwSmemMax);
+        return MIA_EINVAL;
+    }
     return MIA_OK;
 }
 
@@ -268,17 +298,15 @@ const char *mia_dwconv2d_last_error(void) { return g_dw_err; }
 
 int mia_dwconv2d_fwd(const void *x, const float *weight, const float *bias, void *y, int batch, int channels, int H, int W, int silu,
                      int dtype, void *cuda_stream) {
-    if (int rc = dw_check(x, batch, channels, H, W, dtype)) return rc;
+    int P;
+    size_t smem;
+    if (int rc = dw_check(x, batch, channels, H, W, dtype, false, P, smem)) return rc;
     if (!weight || !y) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d_fwd: null weight or y"); return MIA_EINVAL; }
     const int es = dtype == MIA_F32 ? 4 : 2, HW = H * W;
     DwArgs a{};
     a.x = x; a.y = y; a.w = weight; a.bias = bias; a.batch = batch; a.C = channels; a.H = H; a.W = W; a.silu = silu;
-    int P = 2048 / HW;
-    if (P < 1) P = 1;
-    if (P > 16) P = 16;
     a.planes_per_block = P;
     a.magic_hw = dw_magic(HW); a.magic_w = dw_magic(W);
-    const size_t smem = ((size_t)P * (H + 2) * (W + 2) + (size_t)P * 12) * sizeof(float) + (size_t)P * HW * es;
     const bool vec = (HW % 4) == 0 && ((((uintptr_t)x | (uintptr_t)y) & (4 * es - 1)) == 0);
     const long long n_planes = (long long)batch * channels;
     long long blocks = (n_planes + P - 1) / P;
@@ -291,7 +319,8 @@ int mia_dwconv2d_fwd(const void *x, const float *weight, const float *bias, void
         void (*kern)(const DwArgs);
         if (vec) kern = silu ? &dwconv2d_fwd_kernel<T, true, 4> : &dwconv2d_fwd_kernel<T, false, 4>;
         else kern = silu ? &dwconv2d_fwd_kernel<T, true, 1> : &dwconv2d_fwd_kernel<T, false, 1>;
-        if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (smem > 48 * 1024)
+            if (const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return (int)e;
         kern<<<(int)blocks, kDwThreads, smem, (cudaStream_t)cuda_stream>>>(a);
         return (int)cudaGetLastError();
     });
@@ -301,25 +330,24 @@ int mia_dwconv2d_fwd(const void *x, const float *weight, const float *bias, void
 
 int mia_dwconv2d_bwd(const void *x, const float *weight, const float *bias, const void *dy, void *dx, float *dweight, float *dbias,
                      int batch, int channels, int H, int W, int silu, int dtype, void *cuda_stream) {
-    if (int rc = dw_check(x, batch, channels, H, W, dtype)) return rc;
+    int P;
+    size_t smem;
+    if (int rc = dw_check(x, batch, channels, H, W, dtype, true, P, smem)) return rc;
     if (!weight || !dy || !dx || !dweight) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d_bwd: null pointer"); return MIA_EINVAL; }
     const int es = dtype == MIA_F32 ? 4 : 2, HW = H * W;
     DwArgs a{};
     a.x = x; a.dy = dy; a.dx = dx; a.w = weight; a.bias = bias; a.dw = dweight; a.dbias = dbias;
     a.batch = batch; a.C = channels; a.H = H; a.W = W; a.silu = silu;
-    int P = 2048 / HW;
-    if (P < 1) P = 1;
-    if (P > batch) P = batch;
     a.planes_per_block = P;
     a.magic_hw = dw_magic(HW); a.magic_w = dw_magic(W);
-    const size_t smem = (size_t)2 * P * (H + 2) * (W + 2) * sizeof(float) + (size_t)P * HW * es;
     const bool vec = (HW % 4) == 0 && ((((uintptr_t)x | (uintptr_t)dy | (uintptr_t)dx) & (4 * es - 1)) == 0);
     const int rc = dw_dispatch(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
         void (*kern)(const DwArgs);
         if (vec) kern = silu ? &dwconv2d_bwd_kernel<T, true, 4> : &dwconv2d_bwd_kernel<T, false, 4>;
         else kern = silu ? &dwconv2d_bwd_kernel<T, true, 1> : &dwconv2d_bwd_kernel<T, false, 1>;
-        if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (smem > 48 * 1024)
+            if (const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return (int)e;
         kern<<<channels, kDwThreads, smem, (cudaStream_t)cuda_stream>>>(a);
         return (int)cudaGetLastError();
     });

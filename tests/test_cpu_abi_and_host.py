@@ -174,6 +174,21 @@ def test_dwconv2d_has_no_cpu_path():
         DWConv2dFn.apply(torch.randn(1, 4, 5, 5), torch.randn(4, 1, 5, 5), None, True)
 
 
+def test_dwconv2d_rejects_planes_that_do_not_fit_without_gpu():
+    """A thin plane whose blocks would need more than the 227 KB of shared memory a block may have is refused by the
+    shape check, before any CUDA call (so the refusal names the limit instead of surfacing as a failed launch)."""
+    lib = _lib()
+    buf = ctypes.create_string_buffer(64)
+    p = ctypes.cast(buf, ctypes.c_void_p)
+    assert lib.mia_dwconv2d_fwd(p, p, None, p, 1, 1, 1, 16384, 1, 0, None) == -1               # fp32 1 x 16384 forward
+    assert lib.mia_dwconv2d_last_error() == (b"dwconv2d_fwd: a 1 x 16384 float32 plane needs 262224 bytes of shared memory "
+                                             b"per block, more than the 232448-byte (227 KB) limit")
+    assert lib.mia_dwconv2d_bwd(p, p, None, p, p, p, None, 2, 1, 4, 4096, 1, 0, None) == -1     # fp32 4 x 4096 backward
+    assert b"262240 bytes" in lib.mia_dwconv2d_last_error() and b"dwconv2d_bwd" in lib.mia_dwconv2d_last_error()
+    assert lib.mia_dwconv2d_bwd(p, p, None, p, p, p, None, 1, 1, 1, 16384, 1, 2, None) == -1    # bf16 1 x 16384 backward
+    assert b"16-bit plane" in lib.mia_dwconv2d_last_error()
+
+
 def test_model_regime_generator_and_oracles_agree():
     """The `model` regime of tests/test_scan_ranges_gpu.py lands where it claims (softplus argument within [-9, 0], A within
     [-32, -0.5]: what SS2D / the ARM mixers initialise), and there the two oracles - the reference's own arithmetic in fp32

@@ -14,6 +14,8 @@ import re
 import pytest
 import torch
 
+from tests.kernel_trace import launched, retry, targs
+
 pytestmark = pytest.mark.gpu
 
 BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
@@ -27,29 +29,13 @@ BWD_KERNELS = [("ss_bwd_cw_kernel<", "cw"), ("ss_bwd_rowsn_kernel<", "rowsn"), (
 SCAN_KERNEL = re.compile(r"\bss_(fwd|bwd|finalize)_\w*kernel<")
 
 
-def _targs(name, prefix):
-    body = name[name.index(prefix) + len(prefix):]
-    depth, args, cur = 1, [], ""
-    for ch in body:
-        depth += ch == "<"
-        depth -= ch == ">"
-        if depth == 0 or (depth == 1 and ch == ","):
-            args.append(cur.strip())
-            cur = ""
-            if depth == 0:
-                return args
-        else:
-            cur += ch
-    raise AssertionError(f"unterminated template arguments in {name!r}")
-
-
 def _family(names, table):
     """The one family all scan kernels in ``names`` belong to: 'cw<g>', '<family>' or '<family>-det' (kDet instances)."""
     fams = set()
     for n in names:
         prefix, fam = next(((p, f) for p, f in table if p in n), (None, None))
         assert prefix is not None, f"unexpected scan kernel {n!r}"
-        args = _targs(n, prefix)
+        args = targs(n, prefix)
         if fam == "cw":
             fam += args[3]
         elif fam in ("fastn", "warp") and prefix.startswith("ss_bwd") and args[-1] == "true":
@@ -60,11 +46,7 @@ def _family(names, table):
 
 
 def _scan_kernels(fn):
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        res = fn()
-        torch.cuda.synchronize()
-    return res, [e.name for e in prof.events() if SCAN_KERNEL.search(e.name)]
+    return launched(fn, SCAN_KERNEL)
 
 
 def _inputs(batch, dim, L, N=1, G=1, ddim=None, dtype=BF16, z=False, layout=None, seed=0):
@@ -148,10 +130,9 @@ def run_plan(shape, out_float, det):
 @pytest.mark.parametrize("case", list(PLANS))
 def test_scan_plan(case):
     shape, out_float, det, want_fwd, want_bwd, want_hblk = PLANS[case]
-    for _ in range(3):   # now and then a profiler session loses kernel records: such a row is taken again
-        kf, kb, kh = run_plan(shape, out_float, det)
-        if len(kf) == (3 if "ss_fwd_chunk_kernel<" in " ".join(kf) else 1) and all(k is None or len(k) == 2 for k in (kb, kh)):
-            break
+    kf, kb, kh = retry(lambda: run_plan(shape, out_float, det),
+                       lambda r: len(r[0]) == (3 if "ss_fwd_chunk_kernel<" in " ".join(r[0]) else 1)
+                       and all(k is None or len(k) == 2 for k in r[1:]))
     assert _family(kf, FWD_KERNELS) == want_fwd, kf
     assert len(kf) == (3 if want_fwd == "chunks" else 1), kf
     for names, want in ((kb, want_bwd), (kh, want_hblk)):

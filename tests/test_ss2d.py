@@ -37,21 +37,104 @@ def test_cuda_cross_scan_merge_match_reference(tag):
     assert torch.equal(ys.grad.cpu(), G[f"{tag}.dys"])
 
 
+# Launch paths of csrc/cross_scan.cu (launch_cs): "vec" (4-element accesses, L % 4 == 0 and 4-element aligned operands,
+# up to 8 planes per block within 200 KB), "staged" (one element per thread, up to 4 planes per block; the merge stages
+# fp32) and "direct" (a plane does not fit: gathers from global memory, grid capped at 132 x 16 blocks).
+# (B, C, H, W[, storage offset of the input in elements]) -> {op: (fp32 path, bf16 / fp16 path)}
+CS_PATHS = {
+    (2, 5, 14, 14): dict(scan=("vec", "vec"), merge=("vec", "vec")),                 # 8 planes per block
+    (1, 3, 7, 9): dict(scan=("staged", "staged"), merge=("staged", "staged")),
+    (1, 2, 80, 80): dict(scan=("vec", "vec"), merge=("vec", "vec")),                 # fp32 merge: 2 planes
+    (3, 1, 1, 6): dict(scan=("staged", "staged"), merge=("staged", "staged")),
+    (1, 9, 56, 56): dict(scan=("vec", "vec"), merge=("vec", "vec")),                 # fp32 merge: 4 planes
+    (1, 3, 7, 7): dict(scan=("staged", "staged"), merge=("staged", "staged")),
+    (2, 3, 3, 1): dict(scan=("staged", "staged"), merge=("staged", "staged")),
+    (1, 4, 128, 128): dict(scan=("vec", "staged"), merge=("staged", "vec")),         # 16-bit merge: 1 plane
+    (2, 12, 256, 256): dict(scan=("direct", "staged"), merge=("direct", "direct")),  # 2.9 grid sweeps
+    (1, 12, 227, 227): dict(scan=("direct", "staged"), merge=("direct", "direct")),  # 1.1 grid sweeps
+    (2, 5, 14, 14, 1): dict(scan=("staged", "staged"), merge=("staged", "staged")),
+    (2, 5, 14, 14, 2): dict(scan=("staged", "staged"), merge=("staged", "staged")),
+}
+CS_KERNEL = r"\bcross_(scan|merge)_(vec_|direct_)?kernel<"
+
+
+def _cs_path(names, op):
+    assert len(names) == 1 and f"cross_{op}_" in names[0], names
+    return "vec" if "_vec_kernel<" in names[0] else "direct" if "_direct_kernel<" in names[0] else "staged"
+
+
+def _on_gpu(t, offset):
+    """``t`` on the GPU, contiguous, its storage starting ``offset`` elements into a buffer."""
+    buf = torch.empty(offset + t.numel(), dtype=t.dtype, device="cuda")
+    buf[offset:].copy_(t.reshape(-1))
+    return buf[offset:].view(t.shape)
+
+
+def cs_kernel_paths():
+    """{case: [scan, merge of CrossScan's gradient, merge, scan of CrossMerge's gradient] kernels} under the profiler, for
+    every case and dtype of test_cuda_cross_scan_merge_vs_oracle."""
+    from medical_image_analysis_b200.vmamba import CrossMerge, CrossScan
+    from tests.kernel_trace import names_of
+    out = {}
+    for shape in CS_PATHS:
+        B, C, H, W, off = (*shape, 0)[:5]
+        for dtype in (torch.float32, torch.bfloat16, torch.float16):
+            rnd = lambda *s: _on_gpu(torch.randn(*s).to(dtype), off)
+            x, ys = rnd(B, C, H, W).requires_grad_(True), rnd(B, 4, C, H, W).requires_grad_(True)
+            xs, y = CrossScan.apply(x), CrossMerge.apply(ys)
+            gxs, gy = rnd(B, 4, C, H * W), rnd(B, C, H * W)
+            out[f"{shape}|{dtype}"] = [names_of(lambda: CrossScan.apply(x), CS_KERNEL),
+                                       names_of(lambda: torch.autograd.grad(xs, x, gxs, retain_graph=True), CS_KERNEL),
+                                       names_of(lambda: CrossMerge.apply(ys), CS_KERNEL),
+                                       names_of(lambda: torch.autograd.grad(y, ys, gy, retain_graph=True), CS_KERNEL)]
+    return out
+
+
+@pytest.fixture(scope="module")
+def cs_paths():
+    from tests.kernel_trace import in_child
+    return in_child("tests.test_ss2d:cs_kernel_paths")
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("shape", [(2, 5, 14, 14), (1, 3, 7, 9), (1, 2, 80, 80), (3, 1, 1, 6)])
-def test_cuda_cross_scan_merge_vs_oracle(shape, dtype):
-    from medical_image_analysis_b200.vmamba import cross_merge_fwd, cross_scan_fwd
-    torch.manual_seed(0)
-    B, C, H, W = shape
-    x = torch.randn(*shape).to(dtype)
-    xs = cross_scan_fwd(x.cuda())
-    assert torch.equal(xs.cpu(), cross_scan_ref(x))
-    ys = torch.randn(B, 4, C, H * W).to(dtype)
-    y = cross_merge_fwd(ys.cuda(), H, W)
-    ref = cross_merge_ref(ys.float(), H, W)
-    tol = 1e-6 if dtype == torch.float32 else 2e-2
-    assert torch.allclose(y.float().cpu(), ref, atol=tol, rtol=tol)
+@pytest.mark.parametrize("shape", list(CS_PATHS))
+def test_cuda_cross_scan_merge_vs_oracle(cs_paths, shape, dtype):
+    """CrossScan / CrossMerge forward and backward against the oracle on float64 values: the scan (a permutation) exactly,
+    the merge (a sum of four, rounded once) by the parity criteria; each call's kernel (recorded in a child process,
+    tests/kernel_trace.py) is the one the path table names."""
+    from medical_image_analysis_b200.vmamba import CrossMerge, CrossScan
+    from tests.parity import cmp_f32, cmp_stored
+    B, C, H, W, off = (*shape, 0)[:5]
+    L = H * W
+    want = {op: paths[0 if dtype == torch.float32 else 1] for op, paths in CS_PATHS[shape].items()}
+    if "direct" in want.values():
+        assert B * C * L > 132 * 16 * 256                       # several sweeps of the capped grid
+    g = torch.Generator().manual_seed(B * C * L + off)
+    rnd = lambda *s: torch.randn(*s, generator=g).to(dtype)
+
+    def merged(got, ys, what):
+        ref = cross_merge_ref(ys.double().view(B, 4, C, L), H, W)
+        if dtype == torch.float32:
+            cmp_f32(got.reshape(B, C, L), ref, what)
+        else:
+            cmp_stored(got.reshape(B, C, L), ref, dtype, what)
+
+    tag = f"cross {shape} {dtype}"
+    x0, gxs0, ys0, gy0 = rnd(B, C, H, W), rnd(B, 4, C, L), rnd(B, 4, C, H, W), rnd(B, C, L)
+    k_scan, k_scan_grad, k_merge, k_merge_grad = cs_paths[f"{shape}|{dtype}"]
+    for names, op in ((k_scan, "scan"), (k_scan_grad, "merge"), (k_merge, "merge"), (k_merge_grad, "scan")):
+        assert _cs_path(names, op) == want[op], names
+    x = _on_gpu(x0, off).requires_grad_(True)
+    xs = CrossScan.apply(x)
+    assert torch.equal(xs.cpu(), cross_scan_ref(x0))
+    (dx,) = torch.autograd.grad(xs, x, _on_gpu(gxs0, off))
+    merged(dx, gxs0, f"{tag} CrossScan dx")
+    ys = _on_gpu(ys0, off).requires_grad_(True)
+    y = CrossMerge.apply(ys)
+    merged(y, ys0, f"{tag} CrossMerge y")
+    (dys,) = torch.autograd.grad(y, ys, _on_gpu(gy0, off))
+    assert torch.equal(dys.cpu(), cross_scan_ref(gy0.view(B, C, H, W)).view(B, 4, C, H, W))
 
 
 @pytest.mark.gpu
