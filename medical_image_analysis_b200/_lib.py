@@ -7,6 +7,8 @@ from __future__ import annotations
 import ctypes
 import os
 
+import torch
+
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libmia_scan.so")
 
@@ -51,6 +53,49 @@ class MiaBdl(ctypes.Structure):
     _fields_ = [("ptr", _vp), ("batch_stride", _i64), ("d_stride", _i64), ("seq_stride", _i64)]
 
 
+_I, _LL, _SZ, _STR = ctypes.c_int, ctypes.c_longlong, ctypes.c_size_t, ctypes.c_char_p
+_SS, _SSU, _BDL = ctypes.POINTER(MiaSSParams), ctypes.POINTER(MiaSSUParams), ctypes.POINTER(MiaBdl)
+_SCAN, _CONV, _CS, _DW, _GEMM = "mia_last_error", "mia_conv_last_error", "mia_cs_last_error", "mia_dwconv2d_last_error", "mia_gemm_last_error"
+
+# Every function include/*.h declares: name -> (argtypes, restype, the getter of its error message or None).  The argtypes
+# of an entry point that launches end with its cuda_stream, which call() supplies.
+ABI = {
+    "mia_abi_version": ([], _I, None),
+    "mia_last_error": ([], _STR, None),
+    "mia_conv_last_error": ([], _STR, None),
+    "mia_cs_last_error": ([], _STR, None),
+    "mia_dwconv2d_last_error": ([], _STR, None),
+    "mia_gemm_last_error": ([], _STR, None),
+    "mia_launch_count": ([], ctypes.c_uint64, None),
+    "mia_ss_chunk_len": ([_I], _I, None),
+    "mia_ss_num_chunks": ([_I], _I, None),
+    "mia_ss_block_state_floats": ([_SS], _SZ, None),
+    "mia_ss_fwd_writes_block_states": ([_SS], _I, None),
+    "mia_selective_scan_fwd": ([_SS, _vp], _I, _SCAN),
+    "mia_selective_scan_bwd_workspace": ([_SS], _SZ, None),
+    "mia_selective_scan_bwd": ([_SS, _vp], _I, _SCAN),
+    "mia_selective_scan_bwd_deterministic_workspace": ([_SS], _SZ, None),
+    "mia_selective_scan_bwd_deterministic": ([_SS, _vp], _I, _SCAN),
+    "mia_cross_scan": ([_vp, _vp] + [_I] * 5 + [_vp], _I, _CS),
+    "mia_cross_merge": ([_vp, _vp] + [_I] * 5 + [_vp], _I, _CS),
+    "mia_silu_gate": ([_vp, _vp, _vp, _LL, _I, _I, _vp], _I, _CS),
+    "mia_causal_conv1d_fwd": ([_vp] * 4 + [_I] * 6 + [_LL] * 4 + [_vp], _I, _CONV),
+    "mia_causal_conv1d_bwd": ([_vp] * 7 + [_I] * 6 + [_LL] * 6 + [_vp], _I, _CONV),
+    "mia_causal_conv1d_fwd_ex": ([_BDL, _vp, _vp, _BDL] + [_I] * 7 + [_vp], _I, _CONV),
+    "mia_causal_conv1d_bwd_ex_workspace": ([_I] * 4, _SZ, None),
+    "mia_causal_conv1d_bwd_ex": ([_BDL, _vp, _vp, _BDL, _I, _BDL, _vp, _vp, _vp, _SZ] + [_I] * 6 + [_vp], _I, _CONV),
+    "mia_silu_gate_fwd_ex": ([_BDL, _I, _BDL, _BDL] + [_I] * 5 + [_vp], _I, _CONV),
+    "mia_silu_gate_bwd_ex": ([_BDL, _BDL, _I, _BDL, _BDL, _I, _BDL] + [_I] * 5 + [_vp], _I, _CONV),
+    "mia_dwconv2d_fwd": ([_vp] * 4 + [_I] * 6 + [_vp], _I, _DW),
+    "mia_dwconv2d_bwd": ([_vp] * 7 + [_I] * 6 + [_vp], _I, _DW),
+    "mia_selective_state_update": ([_SSU, _vp], _I, _SCAN),
+    "mia_causal_conv1d_update": ([_vp] * 5 + [_I] * 8 + [_LL] * 7 + [_vp], _I, _CONV),
+    "mia_gemm_tn": ([_vp] * 4 + [_I] * 3 + [_LL] * 3 + [_I] * 3 + [_vp], _I, _GEMM),
+    "mia_gemm": ([_vp] * 4 + [_I] * 3 + [_LL] * 3 + [_I] * 5 + [_vp], _I, _GEMM),
+}
+
+DTYPE_CODES = {torch.float32: MIA_F32, torch.float16: MIA_F16, torch.bfloat16: MIA_BF16}
+
 _lib = None
 
 
@@ -64,68 +109,32 @@ def lib() -> ctypes.CDLL:
                 "`python -c 'import __graft_entry__ as g; g.build()'` (or `python -m medical_image_analysis_b200._build`). "
                 "There is no CPU / PyTorch fallback for the selective scan.")
         L = ctypes.CDLL(LIB_PATH)
-        L.mia_abi_version.restype = ctypes.c_int
-        L.mia_last_error.restype = ctypes.c_char_p
-        L.mia_launch_count.restype = ctypes.c_uint64
-        L.mia_ss_chunk_len.argtypes = [ctypes.c_int]
-        L.mia_ss_chunk_len.restype = ctypes.c_int
-        L.mia_ss_num_chunks.argtypes = [ctypes.c_int]
-        L.mia_ss_num_chunks.restype = ctypes.c_int
-        L.mia_selective_scan_fwd.argtypes = [ctypes.POINTER(MiaSSParams), _vp]
-        L.mia_selective_scan_fwd.restype = ctypes.c_int
-        L.mia_selective_scan_bwd.argtypes = [ctypes.POINTER(MiaSSParams), _vp]
-        L.mia_selective_scan_bwd.restype = ctypes.c_int
-        L.mia_selective_scan_bwd_workspace.argtypes = [ctypes.POINTER(MiaSSParams)]
-        L.mia_selective_scan_bwd_workspace.restype = ctypes.c_size_t
-        L.mia_selective_scan_bwd_deterministic.argtypes = [ctypes.POINTER(MiaSSParams), _vp]
-        L.mia_selective_scan_bwd_deterministic.restype = ctypes.c_int
-        L.mia_selective_scan_bwd_deterministic_workspace.argtypes = [ctypes.POINTER(MiaSSParams)]
-        L.mia_selective_scan_bwd_deterministic_workspace.restype = ctypes.c_size_t
-        for fn in (L.mia_cross_scan, L.mia_cross_merge):
-            fn.argtypes = [_vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-            fn.restype = ctypes.c_int
-        L.mia_cs_last_error.restype = ctypes.c_char_p
-        L.mia_silu_gate.argtypes = [_vp, _vp, _vp, ctypes.c_longlong, ctypes.c_int, ctypes.c_int, _vp]
-        L.mia_silu_gate.restype = ctypes.c_int
-        ll, ci = ctypes.c_longlong, ctypes.c_int
-        L.mia_causal_conv1d_fwd.argtypes = [_vp, _vp, _vp, _vp, ci, ci, ci, ci, ci, ci, ll, ll, ll, ll, _vp]
-        L.mia_causal_conv1d_fwd.restype = ci
-        L.mia_causal_conv1d_bwd.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, ci, ci, ci, ci, ci, ci, ll, ll, ll, ll, ll, ll, _vp]
-        L.mia_causal_conv1d_bwd.restype = ci
-        L.mia_conv_last_error.restype = ctypes.c_char_p
-        bdl = ctypes.POINTER(MiaBdl)
-        L.mia_causal_conv1d_fwd_ex.argtypes = [bdl, _vp, _vp, bdl, ci, ci, ci, ci, ci, ci, ci, _vp]
-        L.mia_causal_conv1d_fwd_ex.restype = ci
-        L.mia_causal_conv1d_bwd_ex_workspace.argtypes = [ci, ci, ci, ci]
-        L.mia_causal_conv1d_bwd_ex_workspace.restype = ctypes.c_size_t
-        L.mia_causal_conv1d_bwd_ex.argtypes = [bdl, _vp, _vp, bdl, ci, bdl, _vp, _vp, _vp, ctypes.c_size_t, ci, ci, ci, ci, ci, ci, _vp]
-        L.mia_causal_conv1d_bwd_ex.restype = ci
-        L.mia_silu_gate_fwd_ex.argtypes = [bdl, ci, bdl, bdl, ci, ci, ci, ci, ci, _vp]
-        L.mia_silu_gate_fwd_ex.restype = ci
-        L.mia_silu_gate_bwd_ex.argtypes = [bdl, bdl, ci, bdl, bdl, ci, bdl, ci, ci, ci, ci, ci, _vp]
-        L.mia_silu_gate_bwd_ex.restype = ci
-        L.mia_selective_state_update.argtypes = [ctypes.POINTER(MiaSSUParams), _vp]
-        L.mia_selective_state_update.restype = ci
-        L.mia_causal_conv1d_update.argtypes = [_vp, _vp, _vp, _vp, _vp] + [ci] * 8 + [ll] * 7 + [_vp]
-        L.mia_causal_conv1d_update.restype = ci
-        L.mia_dwconv2d_fwd.argtypes = [_vp, _vp, _vp, _vp, ci, ci, ci, ci, ci, ci, _vp]
-        L.mia_dwconv2d_fwd.restype = ci
-        L.mia_dwconv2d_bwd.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, ci, ci, ci, ci, ci, ci, _vp]
-        L.mia_dwconv2d_bwd.restype = ci
-        L.mia_dwconv2d_last_error.restype = ctypes.c_char_p
-        L.mia_gemm_tn.argtypes = [_vp, _vp, _vp, _vp, ci, ci, ci, ll, ll, ll, ci, ci, ci, _vp]
-        L.mia_gemm_tn.restype = ci
-        L.mia_gemm.argtypes = [_vp, _vp, _vp, _vp, ci, ci, ci, ll, ll, ll, ci, ci, ci, ci, ci, _vp]
-        L.mia_gemm.restype = ci
-        L.mia_gemm_last_error.restype = ctypes.c_char_p
-        L.mia_ss_block_state_floats.argtypes = [ctypes.POINTER(MiaSSParams)]
-        L.mia_ss_block_state_floats.restype = ctypes.c_size_t
-        L.mia_ss_fwd_writes_block_states.argtypes = [ctypes.POINTER(MiaSSParams)]
-        L.mia_ss_fwd_writes_block_states.restype = ctypes.c_int
+        for name, (argtypes, restype, _) in ABI.items():
+            fn = getattr(L, name)
+            fn.argtypes, fn.restype = argtypes, restype
         if L.mia_abi_version() != 2:
             raise RuntimeError(f"libmia_scan.so ABI version {L.mia_abi_version()} != 2: rebuild it")
         _lib = L
     return _lib
+
+
+def dtype_code(dtype: torch.dtype) -> int:
+    """MIA_F32 / MIA_F16 / MIA_BF16 of a torch dtype (KeyError for any other)."""
+    return DTYPE_CODES[dtype]
+
+
+def call(name: str, what: str, device, *args) -> None:
+    """The launch path of every entry point: runs ``name(*args, cuda_stream)`` with ``device`` current and its current stream
+    as the trailing cuda_stream, and raises ``RuntimeError(f"{what}: <message> (code <rc>)")`` with the message of the
+    entry point's own error channel when it fails.  device=None passes a null stream and switches no device."""
+    L = lib()
+    if device is None:
+        rc = getattr(L, name)(*args, None)
+    else:
+        with torch.cuda.device(device):
+            rc = getattr(L, name)(*args, torch.cuda.current_stream(device).cuda_stream)
+    if rc != 0:
+        raise RuntimeError(f"{what}: {getattr(L, ABI[name][2])().decode()} (code {rc})")
 
 
 def check(rc: int, what: str) -> None:

@@ -11,11 +11,11 @@
 // registers -> shared memory -> one write: deterministic, no atomics.
 #include <cuda_runtime.h>
 
-#include <cstdio>
 #include <initializer_list>
 #include <type_traits>
 
 #include "../../include/mia_selective_scan.h"
+#include "abi_host.h"
 #include "scan_common.cuh"
 
 namespace {
@@ -232,29 +232,15 @@ __global__ void __launch_bounds__(kConvThreads) causal_conv1d_bwd_kernel(const C
     }
 }
 
-// exact floor(i / d) for 0 <= i with i * d < 2^32 by multiply-high
-uint32_t div_magic(int d) { return d == 1 ? 0u : (uint32_t)((0x100000000ULL + (uint64_t)d - 1) / (uint64_t)d); }
-
-thread_local char g_conv_err[256] = "";
-
 int conv_check(ConvArgs &a, const void *x, int batch, int dim, int L, int width, int dtype, const long long *strides, int nstrides) {
-    if (!x || batch <= 0 || dim <= 0 || L <= 0) { snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d: empty or null input"); return MIA_EINVAL; }
-    if (width < 1 || width > kMaxW) { snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d only supports width between 1 and 4"); return MIA_EINVAL; }
-    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) { snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d: bad dtype"); return MIA_EINVAL; }
-    if (L % 4) { snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d: seqlen must be a multiple of 4 (got %d)", L); return MIA_EINVAL; }
+    if (!x || batch <= 0 || dim <= 0 || L <= 0) return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d: empty or null input");
+    if (width < 1 || width > kMaxW) return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d only supports width between 1 and 4");
+    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d: bad dtype");
+    if (L % 4) return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d: seqlen must be a multiple of 4 (got %d)", L);
     for (int i = 0; i < nstrides; ++i)
-        if (strides[i] % 4) { snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d: batch / channel strides must be multiples of 4 elements"); return MIA_EINVAL; }
+        if (strides[i] % 4) return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d: batch / channel strides must be multiples of 4 elements");
     (void)a;
     return MIA_OK;
-}
-
-template <typename F>
-int conv_dispatch(int dtype, F &&f) {
-    switch (dtype) {
-        case MIA_F32: return f((float *)nullptr);
-        case MIA_F16: return f((__half *)nullptr);
-        default: return f((__nv_bfloat16 *)nullptr);
-    }
 }
 
 template <typename T>
@@ -558,19 +544,18 @@ Op op_of(const mia_bdl *o) { return op_ok(o) ? Op{o->ptr, o->batch_stride, o->d_
 // Checks shared by the four entry points; fills a.in / a.out from the operand arrays.
 int ex_check(const char *what, TileArgs &a, int batch, int dim, int L, int dtype, const mia_bdl *in, int n_in, int min_in,
              const mia_bdl *out, int n_out, int min_out) {
-    if (batch <= 0 || dim <= 0 || L <= 0 || batch > 65535) { snprintf(g_conv_err, sizeof(g_conv_err), "%s: bad sizes", what); return MIA_EINVAL; }
-    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) { snprintf(g_conv_err, sizeof(g_conv_err), "%s: bad dtype", what); return MIA_EINVAL; }
+    if (batch <= 0 || dim <= 0 || L <= 0 || batch > 65535) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: bad sizes", what);
+    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: bad dtype", what);
     if (n_in < min_in || n_in > kMaxOps || n_out < min_out || n_out > kMaxOps || (n_in && !in) || (n_out && !out)) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "%s: %d inputs / %d outputs (at least %d / %d, at most %d each)", what, n_in, n_out,
-                 min_in, min_out, kMaxOps);
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: %d inputs / %d outputs (at least %d / %d, at most %d each)", what, n_in, n_out,
+                         min_in, min_out, kMaxOps);
     }
     for (int i = 0; i < n_in; ++i) {
-        if (!op_ok(in + i)) { snprintf(g_conv_err, sizeof(g_conv_err), "%s: null input operand", what); return MIA_EINVAL; }
+        if (!op_ok(in + i)) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: null input operand", what);
         a.in[i] = op_of(in + i);
     }
     for (int i = 0; i < n_out; ++i) {
-        if (!op_ok(out + i)) { snprintf(g_conv_err, sizeof(g_conv_err), "%s: null output operand", what); return MIA_EINVAL; }
+        if (!op_ok(out + i)) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: null output operand", what);
         a.out[i] = op_of(out + i);
     }
     a.n_in = n_in; a.n_out = n_out; a.batch = batch; a.dim = dim; a.L = L;
@@ -579,23 +564,12 @@ int ex_check(const char *what, TileArgs &a, int batch, int dim, int L, int dtype
 
 int ex_launched(const char *what) {
     const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { snprintf(g_conv_err, sizeof(g_conv_err), "%s launch: %s", what, cudaGetErrorString(e)); return MIA_ECUDA; }
-    return MIA_OK;
+    return e == cudaSuccess ? MIA_OK : mia::fail(mia::kErrConv, MIA_ECUDA, "%s launch: %s", what, cudaGetErrorString(e));
 }
 
 }  // namespace
 
-namespace mia {
-// The decode-step conv (csrc/ssm_step.cu) reports through mia_conv_last_error as well.
-int conv_fail(int code, const char *msg) {
-    snprintf(g_conv_err, sizeof(g_conv_err), "%s", msg);
-    return code;
-}
-}  // namespace mia
-
 extern "C" {
-
-const char *mia_conv_last_error(void) { return g_conv_err; }
 
 int mia_causal_conv1d_fwd(const void *x, const float *weight, const float *bias, void *y, int batch, int dim, int seqlen, int width,
                           int silu, int dtype, long long x_batch_stride, long long x_d_stride, long long y_batch_stride,
@@ -605,32 +579,27 @@ int mia_causal_conv1d_fwd(const void *x, const float *weight, const float *bias,
     if (int rc = conv_check(a, x, batch, dim, seqlen, width, dtype, st, 4)) return rc;
     const int es = dtype == MIA_F32 ? 4 : 2;
     if (!weight || !y || (((uintptr_t)x | (uintptr_t)y) & (4 * es - 1))) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d_fwd: null weight / y or x / y not aligned to 4 elements");
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d_fwd: null weight / y or x / y not aligned to 4 elements");
     }
     a.x = x; a.y = y; a.w = weight; a.bias = bias; a.batch = batch; a.dim = dim; a.L = seqlen; a.width = width; a.silu = silu;
     a.x_bs = x_batch_stride; a.x_ds = x_d_stride; a.y_bs = y_batch_stride; a.y_ds = y_d_stride;
     if (x_d_stride != seqlen || y_d_stride != seqlen) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d_fwd: the channel rows of x and y must be contiguous (stride == seqlen)");
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d_fwd: the channel rows of x and y must be contiguous (stride == seqlen)");
     }
     // rows per block: ~2 passes of kConvUnroll quads per thread
     const int qpr = seqlen / 4;
     int rpb = (2 * kConvUnroll * kConvThreads + qpr - 1) / qpr;
     if (rpb > dim) rpb = dim;
     if ((long long)rpb * qpr * qpr >= (1LL << 32) || batch > 65535) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d: sequence or batch too large");
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d: sequence or batch too large");
     }
     const dim3 grid((dim + rpb - 1) / rpb, batch);
     const size_t smem = (size_t)rpb * (width + 1) * sizeof(float);
-    const int rc = conv_dispatch(dtype, [&](auto *tag) {
+    mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
-        launch_conv_fwd<T>(a, grid, rpb, div_magic(qpr), smem, (cudaStream_t)cuda_stream);
-        return (int)cudaGetLastError();
+        launch_conv_fwd<T>(a, grid, rpb, mia::div_magic(qpr), smem, (cudaStream_t)cuda_stream);
     });
-    if (rc != 0) { snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d_fwd launch: %s", cudaGetErrorString((cudaError_t)rc)); return MIA_ECUDA; }
-    return MIA_OK;
+    return mia::launched(mia::kErrConv, "causal_conv1d_fwd launch");
 }
 
 int mia_causal_conv1d_bwd(const void *x, const float *weight, const float *bias, const void *dy, void *dx, float *dweight, float *dbias,
@@ -642,24 +611,20 @@ int mia_causal_conv1d_bwd(const void *x, const float *weight, const float *bias,
     if (int rc = conv_check(a, x, batch, dim, seqlen, width, dtype, st, 6)) return rc;
     const int es = dtype == MIA_F32 ? 4 : 2;
     if (!weight || !dy || !dx || !dweight || (((uintptr_t)x | (uintptr_t)dy | (uintptr_t)dx) & (4 * es - 1))) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d_bwd: null pointer or x / dy / dx not aligned to 4 elements");
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d_bwd: null pointer or x / dy / dx not aligned to 4 elements");
     }
     a.x = x; a.dy = dy; a.dx = dx; a.w = weight; a.bias = bias; a.dw = dweight; a.dbias = dbias;
     a.batch = batch; a.dim = dim; a.L = seqlen; a.width = width; a.silu = silu;
     a.x_bs = x_batch_stride; a.x_ds = x_d_stride; a.dy_bs = dy_batch_stride; a.dy_ds = dy_d_stride; a.dx_bs = dx_batch_stride; a.dx_ds = dx_d_stride;
     const int qpr = seqlen / 4;
     if ((long long)batch * qpr * qpr >= (1LL << 32)) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d: batch * sequence too large");
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d: batch * sequence too large");
     }
-    const int rc = conv_dispatch(dtype, [&](auto *tag) {
+    mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
-        launch_conv_bwd<T>(a, div_magic(qpr), (cudaStream_t)cuda_stream);
-        return (int)cudaGetLastError();
+        launch_conv_bwd<T>(a, mia::div_magic(qpr), (cudaStream_t)cuda_stream);
     });
-    if (rc != 0) { snprintf(g_conv_err, sizeof(g_conv_err), "causal_conv1d_bwd launch: %s", cudaGetErrorString((cudaError_t)rc)); return MIA_ECUDA; }
-    return MIA_OK;
+    return mia::launched(mia::kErrConv, "causal_conv1d_bwd launch");
 }
 
 // ---- the fused inner block's kernels (see "tile kernels" above)
@@ -669,18 +634,16 @@ int mia_causal_conv1d_fwd_ex(const mia_bdl *x, const float *weight, const float 
     TileArgs a{};
     if (int rc = ex_check(what, a, batch, dim, seqlen, dtype, nullptr, 0, 0, ys, n_ys, 1)) return rc;
     if (!op_ok(x) || !weight || width < 1 || width > kMaxW) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "%s: x and weight are required, width 1-4", what);
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: x and weight are required, width 1-4", what);
     }
     a.x = op_of(x); a.w = weight; a.bias = bias;
     const dim3 grid((dim + kTC - 1) / kTC, (seqlen + kTT - 1) / kTT, batch);
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    conv_dispatch(dtype, [&](auto *tag) {
+    mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
 #define MIA_EX_FWD(W) (silu ? conv_fwd_ex_kernel<T, W, true><<<grid, kTileThreads, 0, st>>>(a) : conv_fwd_ex_kernel<T, W, false><<<grid, kTileThreads, 0, st>>>(a))
         switch (width) { case 4: MIA_EX_FWD(4); break; case 3: MIA_EX_FWD(3); break; case 2: MIA_EX_FWD(2); break; default: MIA_EX_FWD(1); }
 #undef MIA_EX_FWD
-        return 0;
     });
     return ex_launched(what);
 }
@@ -697,23 +660,20 @@ int mia_causal_conv1d_bwd_ex(const mia_bdl *x, const float *weight, const float 
     TileArgs a{};
     if (int rc = ex_check(what, a, batch, dim, seqlen, dtype, dys, n_dys, 1, nullptr, 0, 0)) return rc;
     if (!op_ok(x) || !op_ok(dx) || !weight || !dweight || width < 1 || width > kMaxW) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "%s: x, dx, weight and dweight are required, width 1-4", what);
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: x, dx, weight and dweight are required, width 1-4", what);
     }
     if (!workspace || workspace_bytes < mia_causal_conv1d_bwd_ex_workspace(batch, dim, seqlen, width)) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "%s: workspace missing or too small", what);
-        return MIA_EWORKSPACE;
+        return mia::fail(mia::kErrConv, MIA_EWORKSPACE, "%s: workspace missing or too small", what);
     }
     a.x = op_of(x); a.dx = op_of(dx); a.w = weight; a.bias = bias; a.dw = dweight; a.dbias = dbias; a.part = (float *)workspace;
     a.n_tt = (seqlen + kTT - 1) / kTT; a.parts = conv_bwd_ex_parts(batch, dim, seqlen);
     const dim3 grid((dim + kTC - 1) / kTC, a.parts);
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    conv_dispatch(dtype, [&](auto *tag) {
+    mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
 #define MIA_EX_BWD(W) (silu ? conv_bwd_ex_kernel<T, W, true><<<grid, kTileThreads, 0, st>>>(a) : conv_bwd_ex_kernel<T, W, false><<<grid, kTileThreads, 0, st>>>(a))
         switch (width) { case 4: MIA_EX_BWD(4); break; case 3: MIA_EX_BWD(3); break; case 2: MIA_EX_BWD(2); break; default: MIA_EX_BWD(1); }
 #undef MIA_EX_BWD
-        return 0;
     });
     if (int rc = ex_launched(what)) return rc;
     conv_bwd_ex_finalize<<<(dim * (width + 1) + 255) / 256, 256, 0, st>>>(a, width);
@@ -725,13 +685,12 @@ int mia_silu_gate_fwd_ex(const mia_bdl *outs, int n_outs, const mia_bdl *z, cons
     const char *what = "silu_gate_fwd_ex";
     TileArgs a{};
     if (int rc = ex_check(what, a, batch, dim, seqlen, dtype, outs, n_outs, 1, out_zs, n_out_zs, 1)) return rc;
-    if (!op_ok(z)) { snprintf(g_conv_err, sizeof(g_conv_err), "%s: z is required", what); return MIA_EINVAL; }
+    if (!op_ok(z)) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: z is required", what);
     a.z = op_of(z);
     const dim3 grid((dim + kTC - 1) / kTC, (seqlen + kTT - 1) / kTT, batch);
-    conv_dispatch(dtype, [&](auto *tag) {
+    mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
         gate_fwd_ex_kernel<T><<<grid, kTileThreads, 0, (cudaStream_t)cuda_stream>>>(a);
-        return 0;
     });
     return ex_launched(what);
 }
@@ -740,14 +699,12 @@ int mia_silu_gate_bwd_ex(const mia_bdl *dy, const mia_bdl *outs, int n_outs, con
                          int batch, int dim, int seqlen, int dtype, int dout_dtype, void *cuda_stream) {
     const char *what = "silu_gate_bwd_ex";
     if (dout_dtype != dtype && dout_dtype != MIA_F32) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "%s: douts must have the call's dtype or float32", what);
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: douts must have the call's dtype or float32", what);
     }
     TileArgs a{};
     mia_bdl in[kMaxOps];
     if (!op_ok(dy) || !op_ok(z) || !op_ok(dz) || !outs || n_outs < 1 || n_outs > kMaxOps - 1) {
-        snprintf(g_conv_err, sizeof(g_conv_err), "%s: dy, z, dz and 1-%d outs are required", what, kMaxOps - 1);
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: dy, z, dz and 1-%d outs are required", what, kMaxOps - 1);
     }
     in[0] = *dy;
     for (int i = 0; i < n_outs; ++i) in[1 + i] = outs[i];
@@ -755,15 +712,14 @@ int mia_silu_gate_bwd_ex(const mia_bdl *dy, const mia_bdl *outs, int n_outs, con
     a.z = op_of(z); a.dz = op_of(dz);
     const dim3 grid((dim + kTC - 1) / kTC, (seqlen + kTT - 1) / kTT, batch);
     const int smem = 3 * kTC * (kTT + 1) * (int)sizeof(float);
-    const int rc = conv_dispatch(dtype, [&](auto *tag) {
+    const cudaError_t e = mia::dispatch_dtype<cudaError_t>(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
         auto k = dout_dtype == MIA_F32 ? gate_bwd_ex_kernel<T, float> : gate_bwd_ex_kernel<T, T>;
         const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return (int)e;
-        k<<<grid, kTileThreads, smem, (cudaStream_t)cuda_stream>>>(a);
-        return 0;
+        if (e == cudaSuccess) k<<<grid, kTileThreads, smem, (cudaStream_t)cuda_stream>>>(a);
+        return e;
     });
-    if (rc) { snprintf(g_conv_err, sizeof(g_conv_err), "%s: %s", what, cudaGetErrorString((cudaError_t)rc)); return MIA_ECUDA; }
+    if (int rc = mia::cuda_fail(mia::kErrConv, what, e)) return rc;
     return ex_launched(what);
 }
 

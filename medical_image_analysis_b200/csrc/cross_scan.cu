@@ -7,9 +7,10 @@
 // 4 reads + 1 write (merge) per element.
 #include <cuda_runtime.h>
 
-#include <cstdio>
+#include <type_traits>
 
 #include "../../include/mia_selective_scan.h"
+#include "abi_host.h"
 #include "scan_common.cuh"
 
 namespace {
@@ -212,16 +213,30 @@ __global__ void __launch_bounds__(256) silu_gate_kernel(const typename mia::Cvt<
     }
 }
 
-uint32_t cs_magic(int d) { return d == 1 ? 0u : (uint32_t)((0x100000000ULL + (uint64_t)d - 1) / (uint64_t)d); }
+}  // namespace
 
-thread_local char g_cs_err[256] = "";
-int cs_fail(int code, const char *msg) { snprintf(g_cs_err, sizeof(g_cs_err), "%s", msg); return code; }
-int cs_cuda(const char *what) {
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) return MIA_OK;
-    snprintf(g_cs_err, sizeof(g_cs_err), "%s: %s", what, cudaGetErrorString(e));
-    return MIA_ECUDA;
+// Defined ahead of the cross scan's launchers: the gate kernels are instantiated first, which fixes where they sit among
+// the functions of the cubin.
+extern "C" int mia_silu_gate(const void *out, const void *z, void *out_z, long long n, int z_dtype, int out_dtype, void *cuda_stream) {
+    if (!out || !z || !out_z) return mia::fail(mia::kErrCs, MIA_EINVAL, "silu_gate: null pointer");
+    if (n <= 0) return mia::fail(mia::kErrCs, MIA_EINVAL, "silu_gate: empty");
+    if (out_dtype != z_dtype && out_dtype != MIA_F32) return mia::fail(mia::kErrCs, MIA_EINVAL, "silu_gate: out dtype must be z's dtype or float32");
+    if (z_dtype != MIA_F32 && z_dtype != MIA_F16 && z_dtype != MIA_BF16)
+        return mia::fail(mia::kErrCs, MIA_EINVAL, "silu_gate: dtype must be MIA_F32, MIA_F16 or MIA_BF16");
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    long long blocks = (n + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    const int g = (int)blocks;
+#define MIA_GATE(T, TO) silu_gate_kernel<T, TO><<<g, 256, 0, st>>>((const typename mia::Cvt<TO>::raw *)out, (const typename mia::Cvt<T>::raw *)z, (typename mia::Cvt<TO>::raw *)out_z, n)
+    mia::dispatch_dtype(z_dtype, [&](auto *tag) {
+        using T = std::remove_pointer_t<decltype(tag)>;
+        if (out_dtype == MIA_F32) MIA_GATE(T, float); else MIA_GATE(T, T);
+    });
+#undef MIA_GATE
+    return mia::launched(mia::kErrCs, "silu_gate launch");
 }
+
+namespace {
 
 constexpr size_t kCsSmemMax = 200 * 1024;
 
@@ -241,17 +256,17 @@ int launch_cs(bool merge, const void *in, void *out, int B, int C, int H, int W,
         if (merge) {
             auto k = &cross_merge_vec_kernel<T>;
             if (vsmem > 48 * 1024 && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vsmem) != cudaSuccess)
-                return cs_cuda("cross_merge: cudaFuncSetAttribute");
+                return mia::launched(mia::kErrCs, "cross_merge: cudaFuncSetAttribute");
             k<<<grid, kCsThreads, vsmem, stream>>>(reinterpret_cast<const raw *>(in), reinterpret_cast<raw *>(out), n_planes, C, H, W,
-                                                  cs_magic(L / 4), cs_magic(W), cs_magic(C), vplanes);
+                                                  mia::div_magic(L / 4), mia::div_magic(W), mia::div_magic(C), vplanes);
         } else {
             auto k = &cross_scan_vec_kernel<T>;
             if (vsmem > 48 * 1024 && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vsmem) != cudaSuccess)
-                return cs_cuda("cross_scan: cudaFuncSetAttribute");
+                return mia::launched(mia::kErrCs, "cross_scan: cudaFuncSetAttribute");
             k<<<grid, kCsThreads, vsmem, stream>>>(reinterpret_cast<const raw *>(in), reinterpret_cast<raw *>(out), n_planes, C, H, W,
-                                                  cs_magic(L / 4), cs_magic(H), cs_magic(C), vplanes);
+                                                  mia::div_magic(L / 4), mia::div_magic(H), mia::div_magic(C), vplanes);
         }
-        return cs_cuda(merge ? "cross_merge launch" : "cross_scan launch");
+        return mia::launched(mia::kErrCs, merge ? "cross_merge launch" : "cross_scan launch");
     }
     const size_t plane = (size_t)L * (merge ? sizeof(float) : sizeof(raw));
     int planes = (int)(kCsSmemMax / plane);
@@ -262,15 +277,15 @@ int launch_cs(bool merge, const void *in, void *out, int B, int C, int H, int W,
         if (merge) {
             auto k = &cross_merge_kernel<T>;
             if (smem > 48 * 1024 && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-                return cs_cuda("cross_merge: cudaFuncSetAttribute");
+                return mia::launched(mia::kErrCs, "cross_merge: cudaFuncSetAttribute");
             k<<<grid, kCsThreads, smem, stream>>>(reinterpret_cast<const raw *>(in), reinterpret_cast<raw *>(out), n_planes, C, H, W, planes);
         } else {
             auto k = &cross_scan_kernel<T>;
             if (smem > 48 * 1024 && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-                return cs_cuda("cross_scan: cudaFuncSetAttribute");
+                return mia::launched(mia::kErrCs, "cross_scan: cudaFuncSetAttribute");
             k<<<grid, kCsThreads, smem, stream>>>(reinterpret_cast<const raw *>(in), reinterpret_cast<raw *>(out), n_planes, C, H, W, planes);
         }
-        return cs_cuda(merge ? "cross_merge launch" : "cross_scan launch");
+        return mia::launched(mia::kErrCs, merge ? "cross_merge launch" : "cross_scan launch");
     }
     // a single plane exceeds shared memory: direct gathers
     const long long total = (long long)n_planes * L;
@@ -278,20 +293,18 @@ int launch_cs(bool merge, const void *in, void *out, int B, int C, int H, int W,
     if (blocks > 132 * 16) blocks = 132 * 16;
     if (merge) cross_merge_direct_kernel<T><<<(int)blocks, kCsThreads, 0, stream>>>(reinterpret_cast<const raw *>(in), reinterpret_cast<raw *>(out), total, C, H, W);
     else cross_scan_direct_kernel<T><<<(int)blocks, kCsThreads, 0, stream>>>(reinterpret_cast<const raw *>(in), reinterpret_cast<raw *>(out), total, C, H, W);
-    return cs_cuda(merge ? "cross_merge (direct) launch" : "cross_scan (direct) launch");
+    return mia::launched(mia::kErrCs, merge ? "cross_merge (direct) launch" : "cross_scan (direct) launch");
 }
 
 int cs_dispatch(bool merge, const void *in, void *out, int B, int C, int H, int W, int dtype, void *stream) {
-    if (!in || !out) return cs_fail(MIA_EINVAL, "cross scan / merge: null pointer");
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return cs_fail(MIA_EINVAL, "cross scan / merge: empty or negative size");
-    if ((long long)H * W > (1LL << 30)) return cs_fail(MIA_EINVAL, "cross scan / merge: H * W too large");
-    cudaStream_t st = (cudaStream_t)stream;
-    switch (dtype) {
-        case MIA_F32: return launch_cs<float>(merge, in, out, B, C, H, W, st);
-        case MIA_F16: return launch_cs<__half>(merge, in, out, B, C, H, W, st);
-        case MIA_BF16: return launch_cs<__nv_bfloat16>(merge, in, out, B, C, H, W, st);
-        default: return cs_fail(MIA_EINVAL, "cross scan / merge: dtype must be MIA_F32, MIA_F16 or MIA_BF16");
-    }
+    if (!in || !out) return mia::fail(mia::kErrCs, MIA_EINVAL, "cross scan / merge: null pointer");
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return mia::fail(mia::kErrCs, MIA_EINVAL, "cross scan / merge: empty or negative size");
+    if ((long long)H * W > (1LL << 30)) return mia::fail(mia::kErrCs, MIA_EINVAL, "cross scan / merge: H * W too large");
+    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16)
+        return mia::fail(mia::kErrCs, MIA_EINVAL, "cross scan / merge: dtype must be MIA_F32, MIA_F16 or MIA_BF16");
+    return mia::dispatch_dtype<int>(dtype, [&](auto *tag) {
+        return launch_cs<std::remove_pointer_t<decltype(tag)>>(merge, in, out, B, C, H, W, (cudaStream_t)stream);
+    });
 }
 
 }  // namespace
@@ -303,24 +316,4 @@ int mia_cross_scan(const void *x, void *xs, int batch, int channels, int H, int 
 int mia_cross_merge(const void *ys, void *y, int batch, int channels, int H, int W, int dtype, void *cuda_stream) {
     return cs_dispatch(true, ys, y, batch, channels, H, W, dtype, cuda_stream);
 }
-const char *mia_cs_last_error(void) { return g_cs_err; }
-
-int mia_silu_gate(const void *out, const void *z, void *out_z, long long n, int z_dtype, int out_dtype, void *cuda_stream) {
-    if (!out || !z || !out_z) return cs_fail(MIA_EINVAL, "silu_gate: null pointer");
-    if (n <= 0) return cs_fail(MIA_EINVAL, "silu_gate: empty");
-    if (out_dtype != z_dtype && out_dtype != MIA_F32) return cs_fail(MIA_EINVAL, "silu_gate: out dtype must be z's dtype or float32");
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    long long blocks = (n + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    const int g = (int)blocks;
-#define MIA_GATE(T, TO) silu_gate_kernel<T, TO><<<g, 256, 0, st>>>((const typename mia::Cvt<TO>::raw *)out, (const typename mia::Cvt<T>::raw *)z, (typename mia::Cvt<TO>::raw *)out_z, n)
-    switch (z_dtype) {
-        case MIA_F32: MIA_GATE(float, float); break;
-        case MIA_F16: if (out_dtype == MIA_F32) MIA_GATE(__half, float); else MIA_GATE(__half, __half); break;
-        case MIA_BF16: if (out_dtype == MIA_F32) MIA_GATE(__nv_bfloat16, float); else MIA_GATE(__nv_bfloat16, __nv_bfloat16); break;
-        default: return cs_fail(MIA_EINVAL, "silu_gate: dtype must be MIA_F32, MIA_F16 or MIA_BF16");
-    }
-#undef MIA_GATE
-    return cs_cuda("silu_gate launch");
-}
-}
+}  // extern "C"

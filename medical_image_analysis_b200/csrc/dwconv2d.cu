@@ -10,10 +10,10 @@
 // deterministic, no atomics.
 #include <cuda_runtime.h>
 
-#include <cstdio>
 #include <type_traits>
 
 #include "../../include/mia_selective_scan.h"
+#include "abi_host.h"
 #include "scan_common.cuh"
 
 namespace {
@@ -253,9 +253,6 @@ __global__ void __launch_bounds__(kDwThreads) dwconv2d_bwd_kernel(const DwArgs a
     }
 }
 
-thread_local char g_dw_err[256] = "";
-uint32_t dw_magic(int d) { return d == 1 ? 0u : (uint32_t)((0x100000000ULL + (uint64_t)d - 1) / (uint64_t)d); }
-
 constexpr size_t kDwSmemMax = 227 * 1024;   // sm_90's opt-in limit of dynamic shared memory per block
 
 size_t dw_bwd_smem(int P, int H, int W, int es) { return (size_t)2 * P * (H + 2) * (W + 2) * sizeof(float) + (size_t)P * H * W * es; }
@@ -264,68 +261,54 @@ size_t dw_bwd_smem(int P, int H, int W, int es) { return (size_t)2 * P * (H + 2)
 // per pass) and the dynamic shared memory they take.  Thin planes do not fit (a 1 x 16384 fp32 forward, a 4 x 4096 fp32
 // backward): they are rejected here, before any CUDA call.
 int dw_check(const void *x, int batch, int C, int H, int W, int dtype, bool bwd, int &P, size_t &smem) {
-    if (!x || batch <= 0 || C <= 0 || H <= 0 || W <= 0) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d: empty or null input"); return MIA_EINVAL; }
-    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d: bad dtype"); return MIA_EINVAL; }
-    if ((long long)H * W > 16384) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d: planes larger than 16384 elements are not supported"); return MIA_EINVAL; }
-    if ((long long)batch * C >= (1LL << 31) / 2) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d: batch*channels too large"); return MIA_EINVAL; }
+    if (!x || batch <= 0 || C <= 0 || H <= 0 || W <= 0) return mia::fail(mia::kErrDw, MIA_EINVAL, "dwconv2d: empty or null input");
+    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) return mia::fail(mia::kErrDw, MIA_EINVAL, "dwconv2d: bad dtype");
+    if ((long long)H * W > 16384) return mia::fail(mia::kErrDw, MIA_EINVAL, "dwconv2d: planes larger than 16384 elements are not supported");
+    if ((long long)batch * C >= (1LL << 31) / 2) return mia::fail(mia::kErrDw, MIA_EINVAL, "dwconv2d: batch*channels too large");
     const int es = dtype == MIA_F32 ? 4 : 2;
     P = 2048 / (H * W);
     if (P < 1) P = 1;
     if (P > (bwd ? batch : 16)) P = bwd ? batch : 16;
     smem = bwd ? dw_bwd_smem(P, H, W, es) : dw_fwd_smem(P, H, W, es).bytes;
     if (smem > kDwSmemMax) {
-        snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d_%s: a %d x %d %s plane needs %zu bytes of shared memory per block, more than the "
-                 "%zu-byte (227 KB) limit", bwd ? "bwd" : "fwd", H, W, es == 4 ? "float32" : "16-bit", smem, kDwSmemMax);
-        return MIA_EINVAL;
+        return mia::fail(mia::kErrDw, MIA_EINVAL, "dwconv2d_%s: a %d x %d %s plane needs %zu bytes of shared memory per block, "
+                         "more than the %zu-byte (227 KB) limit", bwd ? "bwd" : "fwd", H, W, es == 4 ? "float32" : "16-bit", smem, kDwSmemMax);
     }
     return MIA_OK;
-}
-
-template <typename F>
-int dw_dispatch(int dtype, F &&f) {
-    switch (dtype) {
-        case MIA_F32: return f((float *)nullptr);
-        case MIA_F16: return f((__half *)nullptr);
-        default: return f((__nv_bfloat16 *)nullptr);
-    }
 }
 
 }  // namespace
 
 extern "C" {
 
-const char *mia_dwconv2d_last_error(void) { return g_dw_err; }
-
 int mia_dwconv2d_fwd(const void *x, const float *weight, const float *bias, void *y, int batch, int channels, int H, int W, int silu,
                      int dtype, void *cuda_stream) {
     int P;
     size_t smem;
     if (int rc = dw_check(x, batch, channels, H, W, dtype, false, P, smem)) return rc;
-    if (!weight || !y) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d_fwd: null weight or y"); return MIA_EINVAL; }
+    if (!weight || !y) return mia::fail(mia::kErrDw, MIA_EINVAL, "dwconv2d_fwd: null weight or y");
     const int es = dtype == MIA_F32 ? 4 : 2, HW = H * W;
     DwArgs a{};
     a.x = x; a.y = y; a.w = weight; a.bias = bias; a.batch = batch; a.C = channels; a.H = H; a.W = W; a.silu = silu;
     a.planes_per_block = P;
-    a.magic_hw = dw_magic(HW); a.magic_w = dw_magic(W);
+    a.magic_hw = mia::div_magic(HW); a.magic_w = mia::div_magic(W);
     const bool vec = (HW % 4) == 0 && ((((uintptr_t)x | (uintptr_t)y) & (4 * es - 1)) == 0);
     const long long n_planes = (long long)batch * channels;
     long long blocks = (n_planes + P - 1) / P;
-    int sms = 132, dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (blocks > (long long)sms * 16) blocks = (long long)sms * 16;
-    const int rc = dw_dispatch(dtype, [&](auto *tag) {
+    mia::DeviceInfo di;
+    if (int rc = mia::device_info(mia::kErrDw, di)) return rc;
+    if (blocks > (long long)di.sms * 16) blocks = (long long)di.sms * 16;
+    const cudaError_t e = mia::dispatch_dtype<cudaError_t>(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
         void (*kern)(const DwArgs);
         if (vec) kern = silu ? &dwconv2d_fwd_kernel<T, true, 4> : &dwconv2d_fwd_kernel<T, false, 4>;
         else kern = silu ? &dwconv2d_fwd_kernel<T, true, 1> : &dwconv2d_fwd_kernel<T, false, 1>;
         if (smem > 48 * 1024)
-            if (const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return (int)e;
+            if (const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return e;
         kern<<<(int)blocks, kDwThreads, smem, (cudaStream_t)cuda_stream>>>(a);
-        return (int)cudaGetLastError();
+        return cudaGetLastError();
     });
-    if (rc != 0) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d_fwd launch: %s", cudaGetErrorString((cudaError_t)rc)); return MIA_ECUDA; }
-    return MIA_OK;
+    return mia::cuda_fail(mia::kErrDw, "dwconv2d_fwd launch", e);
 }
 
 int mia_dwconv2d_bwd(const void *x, const float *weight, const float *bias, const void *dy, void *dx, float *dweight, float *dbias,
@@ -333,26 +316,25 @@ int mia_dwconv2d_bwd(const void *x, const float *weight, const float *bias, cons
     int P;
     size_t smem;
     if (int rc = dw_check(x, batch, channels, H, W, dtype, true, P, smem)) return rc;
-    if (!weight || !dy || !dx || !dweight) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d_bwd: null pointer"); return MIA_EINVAL; }
+    if (!weight || !dy || !dx || !dweight) return mia::fail(mia::kErrDw, MIA_EINVAL, "dwconv2d_bwd: null pointer");
     const int es = dtype == MIA_F32 ? 4 : 2, HW = H * W;
     DwArgs a{};
     a.x = x; a.dy = dy; a.dx = dx; a.w = weight; a.bias = bias; a.dw = dweight; a.dbias = dbias;
     a.batch = batch; a.C = channels; a.H = H; a.W = W; a.silu = silu;
     a.planes_per_block = P;
-    a.magic_hw = dw_magic(HW); a.magic_w = dw_magic(W);
+    a.magic_hw = mia::div_magic(HW); a.magic_w = mia::div_magic(W);
     const bool vec = (HW % 4) == 0 && ((((uintptr_t)x | (uintptr_t)dy | (uintptr_t)dx) & (4 * es - 1)) == 0);
-    const int rc = dw_dispatch(dtype, [&](auto *tag) {
+    const cudaError_t e = mia::dispatch_dtype<cudaError_t>(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
         void (*kern)(const DwArgs);
         if (vec) kern = silu ? &dwconv2d_bwd_kernel<T, true, 4> : &dwconv2d_bwd_kernel<T, false, 4>;
         else kern = silu ? &dwconv2d_bwd_kernel<T, true, 1> : &dwconv2d_bwd_kernel<T, false, 1>;
         if (smem > 48 * 1024)
-            if (const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return (int)e;
+            if (const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return e;
         kern<<<channels, kDwThreads, smem, (cudaStream_t)cuda_stream>>>(a);
-        return (int)cudaGetLastError();
+        return cudaGetLastError();
     });
-    if (rc != 0) { snprintf(g_dw_err, sizeof(g_dw_err), "dwconv2d_bwd launch: %s", cudaGetErrorString((cudaError_t)rc)); return MIA_ECUDA; }
-    return MIA_OK;
+    return mia::cuda_fail(mia::kErrDw, "dwconv2d_bwd launch", e);
 }
 
 }  // extern "C"

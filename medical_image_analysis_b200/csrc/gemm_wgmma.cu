@@ -25,26 +25,16 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
-#include <cstdarg>
-#include <cstdio>
 #include <cstring>
 
 #include "../../include/mia_gemm.h"
+#include "abi_host.h"
 #include "scan_common.cuh"
 
 namespace {
 
 constexpr int kBM = 128, kBK = 64;
 constexpr int kGemmThreads = 384;      // producer warpgroup + two consumer warpgroups
-
-thread_local char g_gemm_err[384] = "";
-int gfail(int code, const char *fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_gemm_err, sizeof(g_gemm_err), fmt, ap);
-    va_end(ap);
-    return code;
-}
 
 struct GemmArgs {
     int M, N, K;
@@ -287,7 +277,7 @@ EncodeTiledFn encode_fn() {
 int make_map(CUtensorMap *tm, const void *ptr, long long rows, long long cols, long long ld, int box_rows, int dt) {
     // rows x cols with cols contiguous; the box is [box_rows][128 bytes of columns]
     EncodeTiledFn fn = encode_fn();
-    if (!fn) return gfail(MIA_GEMM_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    if (!fn) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const int es = dt == MIA_GEMM_F32 ? 4 : 2;
     cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)ld * es};
@@ -297,7 +287,7 @@ int make_map(CUtensorMap *tm, const void *ptr, long long rows, long long cols, l
                                                         : (dt == MIA_GEMM_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     const CUresult r = fn(tm, cdt, 2, const_cast<void *>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return gfail(MIA_GEMM_ECUDA, "cuTensorMapEncodeTiled failed (CUresult %d): rows %lld cols %lld ld %lld", (int)r, rows, cols, ld);
+    if (r != CUDA_SUCCESS) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "cuTensorMapEncodeTiled failed (CUresult %d): rows %lld cols %lld ld %lld", (int)r, rows, cols, ld);
     return MIA_GEMM_OK;
 }
 
@@ -306,34 +296,32 @@ int launch_gemm(const CUtensorMap &tmA, const CUtensorMap &tmB, GemmArgs &g, int
     constexpr int smem = kStages * (kBM * kBK * 2 + BN * kBK * 2) + 2 * kStages * 8 + 1024;
     auto k = &gemm_tn_kernel<BN, kStages, kAMN, kBMN, kF16>;
     if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-        return gfail(MIA_GEMM_ECUDA, "cudaFuncSetAttribute(gemm, %d B): %s", smem, cudaGetErrorString(cudaGetLastError()));
+        return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "cudaFuncSetAttribute(gemm, %d B): %s", smem, cudaGetErrorString(cudaGetLastError()));
     g.num_m_blocks = (g.M + kBM - 1) / kBM;
     g.num_n_blocks = (g.N + BN - 1) / BN;
     g.num_k_blocks = (g.K + kBK - 1) / kBK;
     const int tiles = g.num_m_blocks * g.num_n_blocks;
     const int grid = tiles < sms ? tiles : sms;
     k<<<grid, kGemmThreads, smem, stream>>>(tmA, tmB, g);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return gfail(MIA_GEMM_ECUDA, "gemm launch: %s", cudaGetErrorString(e));
-    return MIA_GEMM_OK;
+    return mia::launched(mia::kErrGemm, "gemm launch");
 }
 
 }  // namespace
 
 static int gemm_impl(const void *A, const void *W, const float *bias, void *C, int M, int N, int K, long long lda, long long ldw, long long ldc,
                      int a_mn, int b_mn, int in_dtype, int out_dtype, int act, void *cuda_stream) {
-    if (!A || !W || !C) return gfail(MIA_GEMM_EINVAL, "gemm: null pointer");
-    if (M <= 0 || N <= 0 || K <= 0) return gfail(MIA_GEMM_EINVAL, "gemm: empty or negative size (M %d, N %d, K %d)", M, N, K);
-    if (in_dtype != MIA_GEMM_BF16 && in_dtype != MIA_GEMM_F16) return gfail(MIA_GEMM_EINVAL, "gemm: inputs must be bf16 or fp16");
-    if (out_dtype != in_dtype && out_dtype != MIA_GEMM_F32) return gfail(MIA_GEMM_EINVAL, "gemm: output must be the input dtype or fp32");
-    if (act < 0 || act > MIA_ACT_SILU) return gfail(MIA_GEMM_EINVAL, "gemm: unknown activation %d", act);
+    if (!A || !W || !C) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm: null pointer");
+    if (M <= 0 || N <= 0 || K <= 0) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm: empty or negative size (M %d, N %d, K %d)", M, N, K);
+    if (in_dtype != MIA_GEMM_BF16 && in_dtype != MIA_GEMM_F16) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm: inputs must be bf16 or fp16");
+    if (out_dtype != in_dtype && out_dtype != MIA_GEMM_F32) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm: output must be the input dtype or fp32");
+    if (act < 0 || act > MIA_ACT_SILU) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm: unknown activation %d", act);
     if ((lda % 8) || (ldw % 8) || lda < (a_mn ? M : K) || ldw < (b_mn ? N : K))
-        return gfail(MIA_GEMM_EINVAL, "gemm: row pitches must cover a row and be multiples of 8 elements (lda %lld, ldw %lld, M %d, N %d, K %d)", lda, ldw, M, N, K);
-    if (((uintptr_t)A | (uintptr_t)W) & 15) return gfail(MIA_GEMM_EINVAL, "gemm: A and W must be 16-byte aligned");
-    if (ldc < N) return gfail(MIA_GEMM_EINVAL, "gemm: ldc < N");
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-        return gfail(MIA_GEMM_ECUDA, "gemm: cannot query the device");
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm: row pitches must cover a row and be multiples of 8 elements (lda %lld, ldw %lld, M %d, N %d, K %d)", lda, ldw, M, N, K);
+    if (((uintptr_t)A | (uintptr_t)W) & 15) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm: A and W must be 16-byte aligned");
+    if (ldc < N) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm: ldc < N");
+    mia::DeviceInfo di;
+    if (mia::device_info(mia::kErrGemm, di) != MIA_OK) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "gemm: cannot query the device");
+    const int sms = di.sms;
     GemmArgs g;
     memset(&g, 0, sizeof(g));
     g.M = M; g.N = N; g.K = K; g.act = act; g.out_f32 = out_dtype == MIA_GEMM_F32; g.has_bias = bias != nullptr; g.bias = bias;
@@ -361,8 +349,6 @@ static int gemm_impl(const void *A, const void *W, const float *bias, void *C, i
 }
 
 extern "C" {
-
-const char *mia_gemm_last_error(void) { return g_gemm_err; }
 
 int mia_gemm_tn(const void *A, const void *W, const float *bias, void *C, int M, int N, int K, long long lda, long long ldw, long long ldc,
                 int in_dtype, int out_dtype, int act, void *cuda_stream) {

@@ -2,15 +2,14 @@
 // selective_scan_oflex.cpp:152-204 / 245-312), tile planning, launches, the finalize kernel that folds the
 // backward's deterministic partials, and the extern "C" surface declared in include/mia_selective_scan.h.
 #include <algorithm>
-#include <atomic>
 #include <initializer_list>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <type_traits>
 
 #include "../../include/mia_selective_scan.h"
+#include "abi_host.h"
 #include "scan_common.cuh"
 #include "scan_bwd_rows.cuh"
 #include "scan_bwd_rowsn.cuh"
@@ -37,21 +36,12 @@ template <typename T> cudaError_t launch_bwd_det(const ScanArgs &, int, cudaStre
 
 namespace {
 
-thread_local char g_err[512] = "";
-std::atomic<uint64_t> g_launches{0};
-
-int fail(int code, const char *fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-    return code;
-}
-
 #define MIA_CHECK(cond, ...) \
-    do { if (!(cond)) return fail(MIA_EINVAL, __VA_ARGS__); } while (0)
+    do { if (!(cond)) return mia::fail(mia::kErrScan, MIA_EINVAL, __VA_ARGS__); } while (0)
 #define MIA_CUDA(expr) \
-    do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return fail(MIA_ECUDA, "%s: %s", #expr, cudaGetErrorString(e__)); } while (0)
+    do { if (int rc__ = mia::cuda_fail(mia::kErrScan, #expr, (expr))) return rc__; } while (0)
+
+using mia::DeviceInfo;
 
 // Debugging knobs (force a kernel family, move the half split) exist only in -DMIA_DEBUG builds; the release library
 // reads no environment variable and has no mode that alters results.
@@ -67,21 +57,6 @@ constexpr int dbg_int(const char *, int dflt) { return dflt; }
 
 int esize(int dt) { return dt == MIA_F32 ? 4 : 2; }
 int round_up(int x, int m) { return (x + m - 1) / m * m; }
-
-struct DeviceInfo { int sms = 0; int smem_optin = 0; };
-int device_info(DeviceInfo &di) {
-    static thread_local int cached_dev = -1;
-    static thread_local DeviceInfo cached;
-    int dev = 0;
-    MIA_CUDA(cudaGetDevice(&dev));
-    if (dev != cached_dev) {
-        MIA_CUDA(cudaDeviceGetAttribute(&cached.sms, cudaDevAttrMultiProcessorCount, dev));
-        MIA_CUDA(cudaDeviceGetAttribute(&cached.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-        cached_dev = dev;
-    }
-    di = cached;
-    return MIA_OK;
-}
 
 int lanes_per_row(int L) {
     if (L > 128) return 32;
@@ -668,14 +643,9 @@ template <typename P> using elem_t = std::remove_pointer_t<P>;
 // counts `n_launches` kernel launches; on failure reports "<what> launch: <error>".
 template <typename F>
 int launch(int itype, const char *what, int n_launches, F &&f) {
-    cudaError_t e;
-    switch (itype) {
-        case MIA_F32: e = f((float *)nullptr); break;
-        case MIA_F16: e = f((__half *)nullptr); break;
-        default: e = f((__nv_bfloat16 *)nullptr); break;
-    }
-    if (e != cudaSuccess) return fail(MIA_ECUDA, "%s launch: %s", what, cudaGetErrorString(e));
-    g_launches.fetch_add(n_launches);
+    const cudaError_t e = mia::dispatch_dtype<cudaError_t>(itype, f);
+    if (e != cudaSuccess) return mia::fail(mia::kErrScan, MIA_ECUDA, "%s launch: %s", what, cudaGetErrorString(e));
+    mia::count_launches(n_launches);
     return MIA_OK;
 }
 
@@ -771,18 +741,10 @@ __global__ void ss_finalize_kernel(const __grid_constant__ FinArgs f) {
 
 }  // namespace
 
-namespace mia {
-// For the other units behind this header's error slot and launch counter (csrc/ssm_step.cu).
-int api_fail(int code, const char *msg) { return fail(code, "%s", msg); }
-void api_count_launch(void) { g_launches.fetch_add(1); }
-}  // namespace mia
-
 // =================================================================================================
 extern "C" {
 
 int mia_abi_version(void) { return MIA_ABI_VERSION; }
-const char *mia_last_error(void) { return g_err; }
-uint64_t mia_launch_count(void) { return g_launches.load(); }
 
 int mia_ss_chunk_len(int seqlen) { return lanes_per_row(seqlen) * mia::kTok; }
 int mia_ss_num_chunks(int seqlen) {
@@ -800,7 +762,7 @@ size_t mia_ss_block_state_floats(const mia_ss_params *pp) {
 int mia_ss_fwd_writes_block_states(const mia_ss_params *pp) {
     if (!pp || !pp->hblk || validate_sizes(*pp) != MIA_OK || !pp->u || !pp->delta || !pp->out) return 0;
     DeviceInfo di;
-    if (device_info(di) != MIA_OK) return 0;
+    if (mia::device_info(mia::kErrScan, di) != MIA_OK) return 0;
     mia::CwFwdArgs rw;
     CUtensorMap tm[3];
     int grid = 0;
@@ -808,13 +770,13 @@ int mia_ss_fwd_writes_block_states(const mia_ss_params *pp) {
 }
 
 int mia_selective_scan_fwd(const mia_ss_params *pp, void *cuda_stream) {
-    if (!pp) return fail(MIA_EINVAL, "null params");
+    if (!pp) return mia::fail(mia::kErrScan, MIA_EINVAL, "null params");
     const mia_ss_params &p = *pp;
     if (int rc = validate_common(p)) return rc;
     MIA_CHECK(p.out && p.x, "out and x must not be null");
     MIA_CHECK(!p.z || p.out_z, "out_z is required when z is given");
     DeviceInfo di;
-    if (int rc = device_info(di)) return rc;
+    if (int rc = mia::device_info(mia::kErrScan, di)) return rc;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     const bool of32 = p.otype == MIA_F32 && p.itype != MIA_F32;
     int grid = 0;
@@ -873,7 +835,7 @@ size_t bwd_workspace(const mia_ss_params *pp, bool det) {
     if (validate_sizes(*pp) != MIA_OK) return 0;     // sizes that the backward itself would reject
     det = det && pp->dstate > 1;
     DeviceInfo di;
-    if (device_info(di) != MIA_OK) { di.sms = 132; di.smem_optin = 232448; }
+    if (mia::device_info(mia::kErrScan, di) != MIA_OK) { di.sms = 132; di.smem_optin = 232448; }
     Plan pl;
     mia::ScanArgs a;
     if (plan_and_layout(*pp, di, true, pl, a, det) != MIA_OK) return 0;
@@ -889,7 +851,7 @@ int *det_status_word() {          // raised by a deterministic-backward wait tha
 #endif
 
 int bwd_impl(const mia_ss_params *pp, void *cuda_stream, bool det) {
-    if (!pp) return fail(MIA_EINVAL, "null params");
+    if (!pp) return mia::fail(mia::kErrScan, MIA_EINVAL, "null params");
     const mia_ss_params &p = *pp;
     if (int rc = validate_common(p)) return rc;
     MIA_CHECK(p.dout && p.du && p.ddelta && p.dA && p.dB && p.dC, "dout, du, ddelta, dA, dB, dC must not be null");
@@ -899,7 +861,7 @@ int bwd_impl(const mia_ss_params *pp, void *cuda_stream, bool det) {
     MIA_CHECK(p.n_chunks == 1 || p.x, "x is required when the sequence spans more than one chunk");
     det = det && p.dstate > 1;
     DeviceInfo di;
-    if (int rc = device_info(di)) return rc;
+    if (int rc = mia::device_info(mia::kErrScan, di)) return rc;
     Plan pl;
     mia::ScanArgs a;
     if (int rc = plan_and_layout(p, di, true, pl, a, det)) return rc;
@@ -910,7 +872,7 @@ int bwd_impl(const mia_ss_params *pp, void *cuda_stream, bool det) {
     a.dz_bs = p.dz_batch_stride; a.dz_ds = p.dz_d_stride;
     const WorkspaceLayout w = workspace_layout(p, pl, di.sms, det);
     if (!p.workspace || p.workspace_bytes < w.total)
-        return fail(MIA_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", w.total, p.workspace ? p.workspace_bytes : (size_t)0);
+        return mia::fail(mia::kErrScan, MIA_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", w.total, p.workspace ? p.workspace_bytes : (size_t)0);
     MIA_CHECK(((uintptr_t)p.workspace & 255) == 0, "workspace must be 256-byte aligned");
     char *ws = (char *)p.workspace;
     a.part_dA = (float *)(ws + w.part_dA); a.part_dD = (float *)(ws + w.part_dD); a.part_dbias = (float *)(ws + w.part_dbias);
@@ -948,7 +910,7 @@ int bwd_impl(const mia_ss_params *pp, void *cuda_stream, bool det) {
         if (a.bc_atomic) {
             MIA_CUDA(cudaMemsetAsync(a.acc_dB, 0, w.acc_bytes, stream));
             MIA_CUDA(cudaMemsetAsync(a.acc_dC, 0, w.acc_bytes, stream));
-            g_launches.fetch_add(2);
+            mia::count_launches(2);
         }
         grid = a.n_seg < di.sms ? a.n_seg : di.sms;
         if (det) {
@@ -995,7 +957,7 @@ int bwd_impl(const mia_ss_params *pp, void *cuda_stream, bool det) {
         int st = 0;
         MIA_CUDA(cudaMemcpyAsync(&st, a.det_status, sizeof(int), cudaMemcpyDeviceToHost, stream));
         MIA_CUDA(cudaStreamSynchronize(stream));
-        if (st) return fail(MIA_ECUDA, "selective_scan_bwd_deterministic: an ordering wait timed out (results are wrong)");
+        if (st) return mia::fail(mia::kErrScan, MIA_ECUDA, "selective_scan_bwd_deterministic: an ordering wait timed out (results are wrong)");
     }
 #endif
     return MIA_OK;

@@ -13,18 +13,11 @@
 // the z path, so a step continues a prefill's last_state with the same numerics.
 #include <cuda_runtime.h>
 
-#include <cstdarg>
-#include <cstdio>
 #include <type_traits>
 
 #include "../../include/mia_selective_scan.h"
+#include "abi_host.h"
 #include "scan_common.cuh"
-
-namespace mia {
-int api_fail(int code, const char *msg);
-void api_count_launch(void);
-int conv_fail(int code, const char *msg);
-}  // namespace mia
 
 namespace {
 
@@ -174,55 +167,21 @@ __global__ void __launch_bounds__(kConvStepThreads) causal_conv1d_update_kernel(
 bool good_dtype(int t) { return t == MIA_F32 || t == MIA_F16 || t == MIA_BF16; }
 int esize(int t) { return t == MIA_F32 ? 4 : 2; }
 
-template <typename F>
-cudaError_t dispatch2(int t1, int t2, F &&f) {
-    auto inner = [&](auto *tag1) {
-        switch (t2) {
-            case MIA_F32: return f(tag1, (float *)nullptr);
-            case MIA_F16: return f(tag1, (__half *)nullptr);
-            default: return f(tag1, (__nv_bfloat16 *)nullptr);
-        }
-    };
-    switch (t1) {
-        case MIA_F32: return inner((float *)nullptr);
-        case MIA_F16: return inner((__half *)nullptr);
-        default: return inner((__nv_bfloat16 *)nullptr);
-    }
-}
-
-int ssu_fail(int code, const char *fmt, ...) {
-    char msg[256];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(msg, sizeof(msg), fmt, ap);
-    va_end(ap);
-    return mia::api_fail(code, msg);
-}
-
-int conv_step_fail(int code, const char *fmt, ...) {
-    char msg[256];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(msg, sizeof(msg), fmt, ap);
-    va_end(ap);
-    return mia::conv_fail(code, msg);
-}
-
 }  // namespace
 
 extern "C" {
 
 int mia_selective_state_update(const mia_ssu_params *pp, void *cuda_stream) {
-    if (!pp) return ssu_fail(MIA_EINVAL, "selective_state_update: null params");
+    if (!pp) return mia::fail(mia::kErrScan, MIA_EINVAL, "selective_state_update: null params");
     const mia_ssu_params &p = *pp;
     if (p.batch <= 0 || p.dim <= 0 || p.batch > 65535)
-        return ssu_fail(MIA_EINVAL, "selective_state_update: batch must be in 1..65535 and dim >= 1 (got %d, %d)", p.batch, p.dim);
+        return mia::fail(mia::kErrScan, MIA_EINVAL, "selective_state_update: batch must be in 1..65535 and dim >= 1 (got %d, %d)", p.batch, p.dim);
     if (p.dstate < 1 || p.dstate > kMaxN)
-        return ssu_fail(MIA_EINVAL, "selective_state_update only supports state dimension <= 256 (got %d)", p.dstate);
+        return mia::fail(mia::kErrScan, MIA_EINVAL, "selective_state_update only supports state dimension <= 256 (got %d)", p.dstate);
     if (!good_dtype(p.state_type) || !good_dtype(p.itype) || (p.D && !good_dtype(p.D_type)) || (p.dt_bias && !good_dtype(p.dt_bias_type)))
-        return ssu_fail(MIA_EINVAL, "selective_state_update: every dtype must be float32, float16 or bfloat16");
+        return mia::fail(mia::kErrScan, MIA_EINVAL, "selective_state_update: every dtype must be float32, float16 or bfloat16");
     if (!p.state || !p.x || !p.dt || !p.A || !p.B || !p.C || !p.out)
-        return ssu_fail(MIA_EINVAL, "selective_state_update: null state / x / dt / A / B / C / out");
+        return mia::fail(mia::kErrScan, MIA_EINVAL, "selective_state_update: null state / x / dt / A / B / C / out");
     const int es = esize(p.state_type);
     const bool vec = (p.dstate * es) % 16 == 0 && (p.state_d_stride * es) % 16 == 0 && (p.state_batch_stride * es) % 16 == 0 &&
                      ((uintptr_t)p.state & 15) == 0;
@@ -239,15 +198,16 @@ int mia_selective_state_update(const mia_ssu_params *pp, void *cuda_stream) {
     a.rows_per_cta = (kStepThreads / 32) << (5 - lpr_log2);
     const dim3 grid((p.dim + a.rows_per_cta - 1) / a.rows_per_cta, p.batch);
     const cudaStream_t st = (cudaStream_t)cuda_stream;
-    const cudaError_t e = dispatch2(p.state_type, p.itype, [&](auto *ts, auto *ti) {
-        using TS = typename std::remove_pointer<decltype(ts)>::type;
-        using TI = typename std::remove_pointer<decltype(ti)>::type;
-        if (vec) ss_step_kernel<TS, TI, true><<<grid, kStepThreads, 0, st>>>(a);
-        else ss_step_kernel<TS, TI, false><<<grid, kStepThreads, 0, st>>>(a);
-        return cudaGetLastError();
+    mia::dispatch_dtype(p.state_type, [&](auto *ts) {
+        mia::dispatch_dtype(p.itype, [&](auto *ti) {
+            using TS = typename std::remove_pointer<decltype(ts)>::type;
+            using TI = typename std::remove_pointer<decltype(ti)>::type;
+            if (vec) ss_step_kernel<TS, TI, true><<<grid, kStepThreads, 0, st>>>(a);
+            else ss_step_kernel<TS, TI, false><<<grid, kStepThreads, 0, st>>>(a);
+        });
     });
-    if (e != cudaSuccess) return ssu_fail(MIA_ECUDA, "selective_state_update launch: %s", cudaGetErrorString(e));
-    mia::api_count_launch();
+    if (int rc = mia::launched(mia::kErrScan, "selective_state_update launch")) return rc;
+    mia::count_launches(1);
     return MIA_OK;
 }
 
@@ -255,12 +215,12 @@ int mia_causal_conv1d_update(const void *x, void *conv_state, const void *weight
                              int width, int silu, int x_dtype, int state_dtype, int weight_dtype, int bias_dtype,
                              long long x_batch_stride, long long state_batch_stride, long long state_d_stride, long long state_w_stride,
                              long long weight_d_stride, long long weight_w_stride, long long out_batch_stride, void *cuda_stream) {
-    if (!x || !conv_state || !weight || !out) return conv_step_fail(MIA_EINVAL, "causal_conv1d_update: null x / conv_state / weight / out");
+    if (!x || !conv_state || !weight || !out) return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d_update: null x / conv_state / weight / out");
     if (batch <= 0 || dim <= 0 || batch > 65535)
-        return conv_step_fail(MIA_EINVAL, "causal_conv1d_update: batch must be in 1..65535 and dim >= 1 (got %d, %d)", batch, dim);
-    if (width < 1 || width > kMaxConvW) return conv_step_fail(MIA_EINVAL, "causal_conv1d_update only supports width between 1 and 4 (got %d)", width);
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d_update: batch must be in 1..65535 and dim >= 1 (got %d, %d)", batch, dim);
+    if (width < 1 || width > kMaxConvW) return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d_update only supports width between 1 and 4 (got %d)", width);
     if (!good_dtype(x_dtype) || !good_dtype(state_dtype) || !good_dtype(weight_dtype) || (bias && !good_dtype(bias_dtype)))
-        return conv_step_fail(MIA_EINVAL, "causal_conv1d_update: every dtype must be float32, float16 or bfloat16");
+        return mia::fail(mia::kErrConv, MIA_EINVAL, "causal_conv1d_update: every dtype must be float32, float16 or bfloat16");
     ConvStepArgs a{};
     a.x = x; a.w = weight; a.bias = bias; a.state = conv_state; a.out = out;
     a.x_bs = x_batch_stride; a.s_bs = state_batch_stride; a.s_ds = state_d_stride; a.s_ws = state_w_stride;
@@ -268,14 +228,15 @@ int mia_causal_conv1d_update(const void *x, void *conv_state, const void *weight
     a.batch = batch; a.dim = dim; a.width = width; a.silu = silu != 0; a.w_type = weight_dtype; a.bias_type = bias_dtype;
     const dim3 grid((dim + kConvStepThreads - 1) / kConvStepThreads, batch);
     const cudaStream_t st = (cudaStream_t)cuda_stream;
-    const cudaError_t e = dispatch2(x_dtype, state_dtype, [&](auto *tx, auto *ts) {
-        using TX = typename std::remove_pointer<decltype(tx)>::type;
-        using TS = typename std::remove_pointer<decltype(ts)>::type;
-        causal_conv1d_update_kernel<TX, TS><<<grid, kConvStepThreads, 0, st>>>(a);
-        return cudaGetLastError();
+    mia::dispatch_dtype(x_dtype, [&](auto *tx) {
+        mia::dispatch_dtype(state_dtype, [&](auto *ts) {
+            using TX = typename std::remove_pointer<decltype(tx)>::type;
+            using TS = typename std::remove_pointer<decltype(ts)>::type;
+            causal_conv1d_update_kernel<TX, TS><<<grid, kConvStepThreads, 0, st>>>(a);
+        });
     });
-    if (e != cudaSuccess) return conv_step_fail(MIA_ECUDA, "causal_conv1d_update launch: %s", cudaGetErrorString(e));
-    mia::api_count_launch();
+    if (int rc = mia::launched(mia::kErrConv, "causal_conv1d_update launch")) return rc;
+    mia::count_launches(1);
     return MIA_OK;
 }
 

@@ -11,19 +11,12 @@ fp32 activations (no autocast) are NOT silently rounded to bf16: they take ``F.l
 """
 from __future__ import annotations
 
-import ctypes
-
 import torch
 import torch.nn.functional as F
 
 from . import _lib
 
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_SILU = 0, 1, 2, 3
-_DT = {torch.float32: _lib.MIA_F32, torch.float16: _lib.MIA_F16, torch.bfloat16: _lib.MIA_BF16}
-
-
-def _stream(t):
-    return ctypes.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
 
 
 def gemm_tn(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, act: int = ACT_NONE, out_dtype=None) -> torch.Tensor:
@@ -50,11 +43,8 @@ def gemm_tn(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, 
     c = torch.empty((M, N), dtype=out_dtype, device=a.device)
     if M == 0 or N == 0:
         return c
-    with torch.cuda.device(a.device):
-        rc = _lib.lib().mia_gemm_tn(a.data_ptr(), w.data_ptr(), None if bias is None else bias.data_ptr(), c.data_ptr(), M, N, K,
-                                    a.stride(0), w.stride(0), c.stride(0), _DT[a.dtype], _DT[out_dtype], int(act), _stream(a))
-    if rc != 0:
-        raise RuntimeError(f"mia_gemm_tn: {_lib.lib().mia_gemm_last_error().decode()} (code {rc})")
+    _lib.call("mia_gemm_tn", "mia_gemm_tn", a.device, a.data_ptr(), w.data_ptr(), None if bias is None else bias.data_ptr(), c.data_ptr(),
+              M, N, K, a.stride(0), w.stride(0), c.stride(0), _lib.dtype_code(a.dtype), _lib.dtype_code(out_dtype), int(act))
     return c
 
 
@@ -74,11 +64,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, a_mn: bool = False, b_mn: bool = Fals
             raise RuntimeError("gemm: operands need a contiguous last dim, a row pitch that is a multiple of 8 and 16-byte alignment")
     out_dtype = out_dtype or a.dtype
     c = torch.empty((M, N), dtype=out_dtype, device=a.device)
-    with torch.cuda.device(a.device):
-        rc = _lib.lib().mia_gemm(a.data_ptr(), b.data_ptr(), None, c.data_ptr(), M, N, K, a.stride(0), b.stride(0), c.stride(0), int(a_mn),
-                                 int(b_mn), _DT[a.dtype], _DT[out_dtype], ACT_NONE, _stream(a))
-    if rc != 0:
-        raise RuntimeError(f"mia_gemm: {_lib.lib().mia_gemm_last_error().decode()} (code {rc})")
+    _lib.call("mia_gemm", "mia_gemm", a.device, a.data_ptr(), b.data_ptr(), None, c.data_ptr(), M, N, K, a.stride(0), b.stride(0),
+              c.stride(0), int(a_mn), int(b_mn), _lib.dtype_code(a.dtype), _lib.dtype_code(out_dtype), ACT_NONE)
     return c
 
 

@@ -14,9 +14,6 @@ import torch
 
 from . import _lib
 
-_DT = {torch.float32: _lib.MIA_F32, torch.float16: _lib.MIA_F16, torch.bfloat16: _lib.MIA_BF16}
-
-
 def _req(cond: bool, msg: str) -> None:
     if not cond:
         raise RuntimeError(msg)
@@ -31,7 +28,7 @@ def num_chunks(seqlen: int) -> int:
 
 
 def _check_inputs(u, delta, A, B, C, D, delta_bias, z):
-    _req(u.dtype in _DT, "u must be float32, float16 or bfloat16")                      # oflex.cpp:154
+    _req(u.dtype in _lib.DTYPE_CODES, "u must be float32, float16 or bfloat16")          # oflex.cpp:154
     _req(A.dtype == torch.float32, "A must be float32")                                 # :155
     _req(delta.dtype == u.dtype and B.dtype == u.dtype and C.dtype == u.dtype, "delta, B, C must have u's dtype")  # :157-159
     for name, t in (("u", u), ("delta", delta), ("A", A), ("B", B), ("C", C)):
@@ -59,7 +56,7 @@ def _check_inputs(u, delta, A, B, C, D, delta_bias, z):
 def _fill_inputs(p, u, delta, A, B, C, D, delta_bias, z, softplus, otype):
     batch, dim, L = u.shape
     p.batch, p.dim, p.seqlen, p.dstate, p.n_groups, p.delta_dim = batch, dim, L, A.shape[1], B.shape[1], delta.shape[1]
-    p.itype, p.otype, p.delta_softplus = _DT[u.dtype], _DT[otype], int(bool(softplus))
+    p.itype, p.otype, p.delta_softplus = _lib.dtype_code(u.dtype), _lib.dtype_code(otype), int(bool(softplus))
     p.n_chunks = num_chunks(L)
     p.u, p.delta, p.A, p.B, p.C = u.data_ptr(), delta.data_ptr(), A.data_ptr(), B.data_ptr(), C.data_ptr()
     p.D, p.delta_bias, p.z = _ptr(D), _ptr(delta_bias), _ptr(z)
@@ -70,10 +67,6 @@ def _fill_inputs(p, u, delta, A, B, C, D, delta_bias, z, softplus, otype):
     p.C_batch_stride, p.C_group_stride, p.C_dstate_stride = C.stride(0), C.stride(1), C.stride(2)
     if z is not None:
         p.z_batch_stride, p.z_d_stride = z.stride(0), z.stride(1)
-
-
-def _stream(t: torch.Tensor) -> ctypes.c_void_p:
-    return ctypes.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
 
 
 def scan_fwd(u, delta, A, B, C, D=None, z=None, delta_bias=None, delta_softplus=False, out_float=False, want_block_states=False):
@@ -101,7 +94,7 @@ def scan_fwd(u, delta, A, B, C, D=None, z=None, delta_bias=None, delta_softplus=
                 p.hblk = hblk.data_ptr()
                 if not _lib.lib().mia_ss_fwd_writes_block_states(ctypes.byref(p)):
                     hblk, p.hblk = None, None            # this shape takes a kernel that does not produce them
-        _lib.check(_lib.lib().mia_selective_scan_fwd(ctypes.byref(p), _stream(u)), "selective_scan_fwd")
+        _lib.call("mia_selective_scan_fwd", "selective_scan_fwd", u.device, ctypes.byref(p))
     return (out, x, out_z, hblk) if want_block_states else (out, x, out_z)
 
 
@@ -151,13 +144,12 @@ def scan_bwd(u, delta, A, B, C, D, z, delta_bias, dout, x, out, delta_softplus, 
         p.dD, p.ddelta_bias = _ptr(dD), _ptr(dbias)
         lib = _lib.lib()
         if torch.are_deterministic_algorithms_enabled():
-            ws_fn, bwd_fn = lib.mia_selective_scan_bwd_deterministic_workspace, lib.mia_selective_scan_bwd_deterministic
-            what = "selective_scan_bwd_deterministic"
+            ws_fn, what = lib.mia_selective_scan_bwd_deterministic_workspace, "selective_scan_bwd_deterministic"
         else:
-            ws_fn, bwd_fn, what = lib.mia_selective_scan_bwd_workspace, lib.mia_selective_scan_bwd, "selective_scan_bwd"
+            ws_fn, what = lib.mia_selective_scan_bwd_workspace, "selective_scan_bwd"
         ws_bytes = int(ws_fn(ctypes.byref(p)))
         ws = torch.empty((max(ws_bytes, 256),), dtype=torch.uint8, device=dev)
         p.workspace, p.workspace_bytes = ws.data_ptr(), ws_bytes
-        _lib.check(bwd_fn(ctypes.byref(p), _stream(u)), what)
+        _lib.call("mia_" + what, what, dev, ctypes.byref(p))
         ws.record_stream(torch.cuda.current_stream(dev))
     return du, ddelta, dA, dB, dC, dD, dbias, dz

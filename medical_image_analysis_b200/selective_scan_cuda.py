@@ -31,16 +31,11 @@ def bwd(u, delta, A, B, C, D=None, z=None, delta_bias=None, dout=None, x=None, o
             dz_new = dz
         res.append(dz_new)
         if recompute_out_z:
-            import ctypes
             import torch
             from . import _lib
             o, zc = out.contiguous(), z.contiguous()
             out_z = torch.empty_like(o)
-            dt = {torch.float32: _lib.MIA_F32, torch.float16: _lib.MIA_F16, torch.bfloat16: _lib.MIA_BF16}
-            with torch.cuda.device(o.device):
-                rc = _lib.lib().mia_silu_gate(o.data_ptr(), zc.data_ptr(), out_z.data_ptr(), o.numel(), dt[zc.dtype], dt[o.dtype],
-                                              ctypes.c_void_p(torch.cuda.current_stream(o.device).cuda_stream))
-            if rc != 0:
-                raise RuntimeError(f"silu_gate: {_lib.lib().mia_cs_last_error().decode()} (code {rc})")
+            _lib.call("mia_silu_gate", "silu_gate", o.device, o.data_ptr(), zc.data_ptr(), out_z.data_ptr(), o.numel(),
+                      _lib.dtype_code(zc.dtype), _lib.dtype_code(o.dtype))
             res.append(out_z)
     return res

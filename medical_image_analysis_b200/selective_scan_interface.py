@@ -21,7 +21,7 @@ import ctypes
 import torch
 import torch.nn.functional as F
 
-from . import selective_scan_cuda, selective_scan_cuda_core, selective_scan_cuda_oflex
+from . import _lib, selective_scan_cuda, selective_scan_cuda_core, selective_scan_cuda_oflex
 
 _fwd = torch.amp.custom_fwd(device_type="cuda")
 _bwd = torch.amp.custom_bwd(device_type="cuda")
@@ -168,9 +168,6 @@ def selective_scan_fn(u, delta, A, B, C, D=None, z=None, delta_bias=None, delta_
 
 # ---------------------------------------------------------------------------------------------------------
 # Fused inner blocks of the Vim / ARM fork of mamba_ssm, composed (mamba_simple.py:665-709 is their definition).
-_CONV_DT = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
-
-
 def _conv_rows(t):
     """(batch, dim, L) view with contiguous channel rows and a batch stride that is a multiple of 4 elements (the first
     half of `xz` qualifies as it is); anything else is made contiguous."""
@@ -185,7 +182,6 @@ class CausalConv1dFn(torch.autograd.Function):
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda")
     def forward(ctx, x, weight, bias, silu):
-        from . import _lib
         if x.dim() != 3 or weight.dim() != 2 or weight.shape[0] != x.shape[1]:
             raise RuntimeError("causal_conv1d_fn: x must be (batch, dim, seqlen) and weight (dim, width)")
         if not x.is_cuda:
@@ -195,11 +191,9 @@ class CausalConv1dFn(torch.autograd.Function):
         b32 = None if bias is None else bias.detach().float().contiguous()
         y = torch.empty(x.shape, device=x.device, dtype=x.dtype)
         B, D, L = x.shape
-        rc = _lib.lib().mia_causal_conv1d_fwd(x.data_ptr(), w32.data_ptr(), 0 if b32 is None else b32.data_ptr(), y.data_ptr(), B, D, L,
-                                              weight.shape[1], int(silu), _CONV_DT[x.dtype], x.stride(0), x.stride(1), y.stride(0),
-                                              y.stride(1), torch.cuda.current_stream(x.device).cuda_stream)
-        if rc != 0:
-            raise RuntimeError(f"causal_conv1d_fwd: {_lib.lib().mia_conv_last_error().decode()} (code {rc})")
+        _lib.call("mia_causal_conv1d_fwd", "causal_conv1d_fwd", x.device, x.data_ptr(), w32.data_ptr(), 0 if b32 is None else b32.data_ptr(),
+                  y.data_ptr(), B, D, L, weight.shape[1], int(silu), _lib.dtype_code(x.dtype), x.stride(0), x.stride(1), y.stride(0),
+                  y.stride(1))
         ctx.save_for_backward(x, w32, b32 if b32 is not None else w32.new_empty(0))
         ctx.silu, ctx.has_bias, ctx.wdtype, ctx.bdtype = bool(silu), bias is not None, weight.dtype, None if bias is None else bias.dtype
         return y
@@ -207,19 +201,15 @@ class CausalConv1dFn(torch.autograd.Function):
     @staticmethod
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, dy):
-        from . import _lib
         x, w32, b32 = ctx.saved_tensors
         dy = _conv_rows(dy.to(x.dtype))
         B, D, L = x.shape
         dx = torch.empty(x.shape, device=x.device, dtype=x.dtype)
         dw = torch.empty_like(w32)
         db = torch.empty(D, device=x.device, dtype=torch.float32) if ctx.has_bias else None
-        rc = _lib.lib().mia_causal_conv1d_bwd(x.data_ptr(), w32.data_ptr(), b32.data_ptr() if ctx.has_bias else 0, dy.data_ptr(), dx.data_ptr(),
-                                              dw.data_ptr(), 0 if db is None else db.data_ptr(), B, D, L, w32.shape[1], int(ctx.silu),
-                                              _CONV_DT[x.dtype], x.stride(0), x.stride(1), dy.stride(0), dy.stride(1), dx.stride(0),
-                                              dx.stride(1), torch.cuda.current_stream(x.device).cuda_stream)
-        if rc != 0:
-            raise RuntimeError(f"causal_conv1d_bwd: {_lib.lib().mia_conv_last_error().decode()} (code {rc})")
+        _lib.call("mia_causal_conv1d_bwd", "causal_conv1d_bwd", x.device, x.data_ptr(), w32.data_ptr(), b32.data_ptr() if ctx.has_bias else 0,
+                  dy.data_ptr(), dx.data_ptr(), dw.data_ptr(), 0 if db is None else db.data_ptr(), B, D, L, w32.shape[1], int(ctx.silu),
+                  _lib.dtype_code(x.dtype), x.stride(0), x.stride(1), dy.stride(0), dy.stride(1), dx.stride(0), dx.stride(1))
         return dx, dw.to(ctx.wdtype), (db.to(ctx.bdtype) if db is not None else None), None
 
 
@@ -250,7 +240,7 @@ def _vec(t, n, what):
     """a (n) parameter read as stored (its own dtype) by the decode-step kernels."""
     if t.shape != (n,):
         raise RuntimeError(f"{what} must have shape ({n},), got {tuple(t.shape)}")
-    if t.dtype not in _CONV_DT:
+    if t.dtype not in _lib.DTYPE_CODES:
         raise RuntimeError(f"{what} must be float32, float16 or bfloat16")
     return t if t.stride(0) == 1 else t.contiguous()
 
@@ -260,7 +250,6 @@ def causal_conv1d_update(x, conv_state, weight, bias=None, activation=None):
     MambaMixer.cuda_kernels_forward): x (batch, dim), conv_state (batch, dim, width <= 4) shifted left in place with x
     written into its last column, weight (dim, width); returns act(bias + sum_k weight[:, k] conv_state[..., k]) in x's
     dtype, computed in fp32 by csrc/ssm_step.cu.  weight / bias / conv_state are read in their own dtypes."""
-    from . import _lib
     if activation not in (None, "silu", "swish"):
         raise NotImplementedError("activation must be None, silu or swish")
     _no_cpu("causal_conv1d_update", x, conv_state, weight, bias)
@@ -272,19 +261,16 @@ def causal_conv1d_update(x, conv_state, weight, bias=None, activation=None):
         raise RuntimeError(f"causal_conv1d_update: conv_state {tuple(conv_state.shape)} / weight {tuple(weight.shape)} do not match "
                            f"x {tuple(x.shape)}")
     for t, what in ((x, "x"), (conv_state, "conv_state"), (weight, "weight")):
-        if t.dtype not in _CONV_DT:
+        if t.dtype not in _lib.DTYPE_CODES:
             raise RuntimeError(f"causal_conv1d_update: {what} must be float32, float16 or bfloat16")
     x = _rows(x)
     bias = None if bias is None else _vec(bias, dim, "causal_conv1d_update: bias")
     out = torch.empty((batch, dim), device=x.device, dtype=x.dtype)
-    L = _lib.lib()
-    rc = L.mia_causal_conv1d_update(x.data_ptr(), conv_state.data_ptr(), weight.data_ptr(), 0 if bias is None else bias.data_ptr(),
-                                    out.data_ptr(), batch, dim, width, int(activation is not None), _CONV_DT[x.dtype],
-                                    _CONV_DT[conv_state.dtype], _CONV_DT[weight.dtype], _CONV_DT[bias.dtype] if bias is not None else 0,
-                                    x.stride(0), conv_state.stride(0), conv_state.stride(1), conv_state.stride(2), weight.stride(0),
-                                    weight.stride(1), out.stride(0), torch.cuda.current_stream(x.device).cuda_stream)
-    if rc != 0:
-        raise RuntimeError(f"causal_conv1d_update: {L.mia_conv_last_error().decode()} (code {rc})")
+    code = _lib.dtype_code
+    _lib.call("mia_causal_conv1d_update", "causal_conv1d_update", x.device, x.data_ptr(), conv_state.data_ptr(), weight.data_ptr(),
+              0 if bias is None else bias.data_ptr(), out.data_ptr(), batch, dim, width, int(activation is not None), code(x.dtype),
+              code(conv_state.dtype), code(weight.dtype), code(bias.dtype) if bias is not None else 0, x.stride(0), conv_state.stride(0),
+              conv_state.stride(1), conv_state.stride(2), weight.stride(0), weight.stride(1), out.stride(0))
     return out
 
 
@@ -297,7 +283,6 @@ def selective_state_update(state, x, dt, A, B, C, D=None, z=None, dt_bias=None, 
 
     Returns out (batch, dim) in x's dtype.  No autograd (as upstream).  Grouped B / C and the Mamba-2 head layout are not
     supported."""
-    from . import _lib
     _no_cpu("selective_state_update", state, x, dt, A, B, C, D, z, dt_bias)
     if state.dim() != 3:
         raise NotImplementedError("selective_state_update: only the (batch, dim, dstate) state layout (no Mamba-2 heads)")
@@ -310,7 +295,7 @@ def selective_state_update(state, x, dt, A, B, C, D=None, z=None, dt_bias=None, 
         raise NotImplementedError(f"selective_state_update: B and C must be (batch, dstate) = {(batch, dstate)} (no grouped B / C)")
     if A.shape != (dim, dstate):
         raise RuntimeError(f"selective_state_update: A must be (dim, dstate) = {(dim, dstate)}")
-    if state.dtype not in _CONV_DT or x.dtype not in _CONV_DT:
+    if state.dtype not in _lib.DTYPE_CODES or x.dtype not in _lib.DTYPE_CODES:
         raise RuntimeError("selective_state_update: state and x must be float32, float16 or bfloat16")
     for t, what in ((dt, "dt"), (B, "B"), (C, "C"), (z, "z")):
         if t is not None and t.dtype != x.dtype:
@@ -323,9 +308,9 @@ def selective_state_update(state, x, dt, A, B, C, D=None, z=None, dt_bias=None, 
     out = torch.empty((batch, dim), device=x.device, dtype=x.dtype)
     p = _lib.MiaSSUParams()
     p.batch, p.dim, p.dstate = batch, dim, dstate
-    p.state_type, p.itype = _CONV_DT[state.dtype], _CONV_DT[x.dtype]
-    p.D_type = _CONV_DT[D.dtype] if D is not None else 0
-    p.dt_bias_type = _CONV_DT[dt_bias.dtype] if dt_bias is not None else 0
+    p.state_type, p.itype = _lib.dtype_code(state.dtype), _lib.dtype_code(x.dtype)
+    p.D_type = _lib.dtype_code(D.dtype) if D is not None else 0
+    p.dt_bias_type = _lib.dtype_code(dt_bias.dtype) if dt_bias is not None else 0
     p.dt_softplus = int(bool(dt_softplus))
     p.state, p.x, p.dt, p.B, p.C, p.A, p.out = (t.data_ptr() for t in (state, x, dt, B, C, A, out))
     p.z = z.data_ptr() if z is not None else None
@@ -336,8 +321,7 @@ def selective_state_update(state, x, dt, A, B, C, D=None, z=None, dt_bias=None, 
     p.z_batch_stride = z.stride(0) if z is not None else 0
     p.out_batch_stride = out.stride(0)
     p.A_d_stride, p.A_dstate_stride = A.stride(0), A.stride(1)
-    _lib.check(_lib.lib().mia_selective_state_update(ctypes.byref(p), torch.cuda.current_stream(x.device).cuda_stream),
-               "selective_state_update")
+    _lib.call("mia_selective_state_update", "selective_state_update", x.device, ctypes.byref(p))
     return out
 
 
@@ -346,7 +330,6 @@ def selective_state_update(state, x, dt, A, B, C, D=None, z=None, dt_bias=None, 
 # csrc/causal_conv1d.cu (mia_*_ex), the projection GEMMs and the CUDA scan.  See DESIGN.md section 3.11.
 def _bdl(t, rev=False):
     """struct mia_bdl of a (batch, dim, seqlen) view (any strides); rev: its time-reversed view."""
-    from . import _lib
     if rev:
         return _lib.MiaBdl(t.data_ptr() + (t.shape[2] - 1) * t.stride(2) * t.element_size(), t.stride(0), t.stride(1), -t.stride(2))
     return _lib.MiaBdl(t.data_ptr(), t.stride(0), t.stride(1), t.stride(2))
@@ -354,19 +337,11 @@ def _bdl(t, rev=False):
 
 def _tm(t, L):
     """struct mia_bdl of a token-major (batch * L, dim) matrix seen as (batch, dim, L)."""
-    from . import _lib
     return _lib.MiaBdl(t.data_ptr(), L * t.stride(0), t.stride(1), t.stride(0))
 
 
 def _ops(*ops):
-    from . import _lib
     return (_lib.MiaBdl * len(ops))(*ops), len(ops)
-
-
-def _conv_call(rc, what):
-    from . import _lib
-    if rc != 0:
-        raise RuntimeError(f"{what}: {_lib.lib().mia_conv_last_error().decode()} (code {rc})")
 
 
 def _tm_buffer(n, d, dtype, dev):
@@ -419,14 +394,13 @@ class MambaInnerFn(torch.autograd.Function):
     @_fwd
     def forward(ctx, xz, conv1d_weight, conv1d_bias, x_proj_weight, delta_proj_weight, out_proj_weight, out_proj_bias, A, A_b, D,
                 delta_bias, B_proj_bias, C_proj_bias, delta_softplus, checkpoint_lvl):
-        from . import _lib
         from .scan_op import scan_fwd
         if checkpoint_lvl not in (0, 1):
             raise ValueError(f"checkpoint_lvl must be 0 or 1, got {checkpoint_lvl!r}")
         if not xz.is_cuda:
             raise RuntimeError("mamba_inner_fn: this build has no CPU path (xz must be a CUDA tensor)")
         T = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled() else xz.dtype
-        if T not in _CONV_DT:
+        if T not in _lib.DTYPE_CODES:
             raise RuntimeError("mamba_inner_fn: xz must be float32, float16 or bfloat16")
         xz = xz.to(T)
         b, d2, L = xz.shape
@@ -445,7 +419,6 @@ class MambaInnerFn(torch.autograd.Function):
         D32 = None if D is None else D.float().contiguous()
         db32 = None if delta_bias is None else delta_bias.float().contiguous()
         bi = A_b is not None
-        lib, stream = _lib.lib(), torch.cuda.current_stream(dev).cuda_stream
         ctx.sizes = (b, d, L, W, R, N, K, T, bi, checkpoint_lvl, delta_softplus)
         ctx.has = (conv1d_bias is not None, out_proj_weight is not None, out_proj_bias is not None, D is not None,
                    delta_bias is not None, B_proj_bias is not None, C_proj_bias is not None)
@@ -468,7 +441,7 @@ class MambaInnerFn(torch.autograd.Function):
             y = torch.empty((b, d, L), dtype=T, device=dev)
             ins, n_in = _ops(_bdl(outs[0]), *([_bdl(outs[1], rev=True)] if bi else []))
             oz, n_oz = _ops(_bdl(y))
-            _conv_call(lib.mia_silu_gate_fwd_ex(ins, n_in, ctypes.byref(_bdl(z)), oz, n_oz, b, d, L, _CONV_DT[T], stream), "silu_gate_fwd")
+            _lib.call("mia_silu_gate_fwd_ex", "silu_gate_fwd", dev, ins, n_in, ctypes.byref(_bdl(z)), oz, n_oz, b, d, L, _lib.dtype_code(T))
         keep = [u, delta] + ([u_rev, delta_r] if bi else []) if checkpoint_lvl == 0 else []
         ctx.n_keep = len(keep)
         ctx.save_for_backward(xz, x_dbl, out_f, Bm, Cm, x_f, w32, cb32, x_proj_weight, delta_proj_weight, out_proj_weight, A, D32, db32,
@@ -481,7 +454,6 @@ class MambaInnerFn(torch.autograd.Function):
     @staticmethod
     def _conv(xz, w32, cb32, ctx, want_cm, want_tm):
         """conv + SiLU of xz's x half in one launch -> (u (b, d, l), its reversed copy (bimamba) | None, u token-major | None)."""
-        from . import _lib
         b, d, L, W, R, N, K, T, bi, _, _ = ctx.sizes
         dev = xz.device
         u = torch.empty((b, d, L), dtype=T, device=dev) if want_cm else None
@@ -490,9 +462,8 @@ class MambaInnerFn(torch.autograd.Function):
         outs = ([_bdl(u)] if u is not None else []) + ([_bdl(u_rev, rev=True)] if u_rev is not None else []) + \
                ([_tm(u_tm, L)] if u_tm is not None else [])
         arr, n = _ops(*outs)
-        _conv_call(_lib.lib().mia_causal_conv1d_fwd_ex(ctypes.byref(_bdl(xz[:, :d])), w32.data_ptr(), None if cb32 is None else cb32.data_ptr(),
-                                                        arr, n, b, d, L, W, 1, _CONV_DT[T], torch.cuda.current_stream(dev).cuda_stream),
-                   "causal_conv1d_fwd_ex")
+        _lib.call("mia_causal_conv1d_fwd_ex", "causal_conv1d_fwd_ex", dev, ctypes.byref(_bdl(xz[:, :d])), w32.data_ptr(),
+                  None if cb32 is None else cb32.data_ptr(), arr, n, b, d, L, W, 1, _lib.dtype_code(T))
         return u, u_rev, u_tm
 
     @staticmethod
@@ -512,18 +483,15 @@ class MambaInnerFn(torch.autograd.Function):
     @staticmethod
     def _gate(outs, z, b, d, L, T, dev):
         """(out_f [+ reversed out_b]) * silu(z) written token-major for out_proj."""
-        from . import _lib
         y_tm = _tm_buffer(b * L, d, T, dev)
         ins, n_in = _ops(_bdl(outs[0]), *([_bdl(outs[1], rev=True)] if len(outs) > 1 else []))
         oz, n_oz = _ops(_tm(y_tm, L))
-        _conv_call(_lib.lib().mia_silu_gate_fwd_ex(ins, n_in, ctypes.byref(_bdl(z)), oz, n_oz, b, d, L, _CONV_DT[T],
-                                                   torch.cuda.current_stream(dev).cuda_stream), "silu_gate_fwd_ex")
+        _lib.call("mia_silu_gate_fwd_ex", "silu_gate_fwd_ex", dev, ins, n_in, ctypes.byref(_bdl(z)), oz, n_oz, b, d, L, _lib.dtype_code(T))
         return y_tm
 
     @staticmethod
     @_bwd
     def backward(ctx, dy):
-        from . import _lib
         from .scan_op import scan_bwd
         b, d, L, W, R, N, K, T, bi, lvl, softplus = ctx.sizes
         has_cb, has_out, has_ob, has_D, has_db, has_Bb, has_Cb = ctx.has
@@ -534,7 +502,6 @@ class MambaInnerFn(torch.autograd.Function):
         out_b, x_b, A_b = rest[:3] if bi else (None, None, None)
         keep = rest[3:] if bi else rest
         dev = xz.device
-        lib, stream = _lib.lib(), torch.cuda.current_stream(dev).cuda_stream
         wx, wdt = x_proj_weight.to(T), delta_proj_weight.to(T)
         # recompute what the level did not keep, with the forward's kernels (same bits)
         if lvl == 0:
@@ -566,8 +533,8 @@ class MambaInnerFn(torch.autograd.Function):
         dout_b = torch.empty((b, d, L), dtype=torch.float32, device=dev) if bi else None
         ins, n_in = _ops(_bdl(out_f), *([_bdl(out_b, rev=True)] if bi else []))
         douts, n_do = _ops(_bdl(dout_f), *([_bdl(dout_b, rev=True)] if bi else []))
-        _conv_call(lib.mia_silu_gate_bwd_ex(ctypes.byref(g), ins, n_in, ctypes.byref(_bdl(z)), douts, n_do, ctypes.byref(_bdl(dxz[:, d:])),
-                                            b, d, L, _CONV_DT[T], _CONV_DT[torch.float32], stream), "silu_gate_bwd_ex")
+        _lib.call("mia_silu_gate_bwd_ex", "silu_gate_bwd_ex", dev, ctypes.byref(g), ins, n_in, ctypes.byref(_bdl(z)), douts, n_do,
+                  ctypes.byref(_bdl(dxz[:, d:])), b, d, L, _lib.dtype_code(T), _lib.MIA_F32)
         g = g_tm = g_cm = None                                                       # transients go as soon as they are used
         du_f, dd_f, dA, dB_f, dC_f, dD, ddb, _ = scan_bwd(u, delta, A, Bm, Cm, D32, None, db32, dout_f, x_f, None, softplus)
         del dout_f, u, delta
@@ -604,10 +571,10 @@ class MambaInnerFn(torch.autograd.Function):
         arr, n = _ops(*dys)
         dw32 = torch.empty_like(w32)
         dcb32 = torch.empty(d, dtype=torch.float32, device=dev) if has_cb else None
-        ws = torch.empty((max(1, int(lib.mia_causal_conv1d_bwd_ex_workspace(b, d, L, W))),), dtype=torch.uint8, device=dev)
-        _conv_call(lib.mia_causal_conv1d_bwd_ex(ctypes.byref(_bdl(xz[:, :d])), w32.data_ptr(), None if cb32 is None else cb32.data_ptr(), arr, n,
-                                                ctypes.byref(_bdl(dxz[:, :d])), dw32.data_ptr(), None if dcb32 is None else dcb32.data_ptr(),
-                                                ws.data_ptr(), ws.numel(), b, d, L, W, 1, _CONV_DT[T], stream), "causal_conv1d_bwd_ex")
+        ws = torch.empty((max(1, int(_lib.lib().mia_causal_conv1d_bwd_ex_workspace(b, d, L, W))),), dtype=torch.uint8, device=dev)
+        _lib.call("mia_causal_conv1d_bwd_ex", "causal_conv1d_bwd_ex", dev, ctypes.byref(_bdl(xz[:, :d])), w32.data_ptr(),
+                  None if cb32 is None else cb32.data_ptr(), arr, n, ctypes.byref(_bdl(dxz[:, :d])), dw32.data_ptr(),
+                  None if dcb32 is None else dcb32.data_ptr(), ws.data_ptr(), ws.numel(), b, d, L, W, 1, _lib.dtype_code(T))
         cw_dtype, cb_dtype, D_dtype, db_dtype, _ = ctx.dtypes
         return (dxz, dw32.view(ctx.conv_shape).to(cw_dtype), None if dcb32 is None else dcb32.to(cb_dtype), d_wx,
                 d_wdt.to(delta_proj_weight.dtype), d_out_w, d_out_b, dA, dA_b, None if dD is None else dD.to(D_dtype),

@@ -14,7 +14,6 @@ class is checked against vectors produced by executing the reference's own modul
 """
 from __future__ import annotations
 
-import ctypes
 import math
 from collections import OrderedDict
 from functools import partial
@@ -28,19 +27,12 @@ from . import _lib
 from . import gemm as _gemm
 from .selective_scan_interface import SelectiveScanCore, SelectiveScanMamba, SelectiveScanOflex
 
-_DT = {torch.float32: _lib.MIA_F32, torch.float16: _lib.MIA_F16, torch.bfloat16: _lib.MIA_BF16}
-
-
-def _cs_call(fn, src: torch.Tensor, dst: torch.Tensor, B: int, C: int, H: int, W: int) -> None:
+def _cs_call(name: str, src: torch.Tensor, dst: torch.Tensor, B: int, C: int, H: int, W: int) -> None:
     if not src.is_cuda:
         raise RuntimeError("CrossScan / CrossMerge need CUDA tensors (there is no CPU fallback)")
-    if src.dtype not in _DT:
+    if src.dtype not in _lib.DTYPE_CODES:
         raise RuntimeError("CrossScan / CrossMerge support float32, float16 and bfloat16")
-    with torch.cuda.device(src.device):
-        stream = ctypes.c_void_p(torch.cuda.current_stream(src.device).cuda_stream)
-        rc = fn(src.data_ptr(), dst.data_ptr(), B, C, H, W, _DT[src.dtype], stream)
-        if rc != 0:
-            raise RuntimeError(f"cross scan/merge: {_lib.lib().mia_cs_last_error().decode()} (code {rc})")
+    _lib.call(name, "cross scan/merge", src.device, src.data_ptr(), dst.data_ptr(), B, C, H, W, _lib.dtype_code(src.dtype))
 
 
 class DWConv2dFn(torch.autograd.Function):
@@ -59,10 +51,8 @@ class DWConv2dFn(torch.autograd.Function):
         b32 = None if bias is None else bias.detach().float().contiguous()
         y = torch.empty_like(x)
         B, C, H, W = x.shape
-        rc = _lib.lib().mia_dwconv2d_fwd(x.data_ptr(), w32.data_ptr(), 0 if b32 is None else b32.data_ptr(), y.data_ptr(), B, C, H, W,
-                                         int(silu), _DT[x.dtype], torch.cuda.current_stream(x.device).cuda_stream)
-        if rc != 0:
-            raise RuntimeError(f"dwconv2d_fwd: {_lib.lib().mia_dwconv2d_last_error().decode()} (code {rc})")
+        _lib.call("mia_dwconv2d_fwd", "dwconv2d_fwd", x.device, x.data_ptr(), w32.data_ptr(), 0 if b32 is None else b32.data_ptr(),
+                  y.data_ptr(), B, C, H, W, int(silu), _lib.dtype_code(x.dtype))
         ctx.save_for_backward(x, w32, b32 if b32 is not None else w32.new_empty(0))
         ctx.silu, ctx.has_bias, ctx.wdtype, ctx.bdtype = bool(silu), bias is not None, weight.dtype, None if bias is None else bias.dtype
         return y
@@ -76,11 +66,9 @@ class DWConv2dFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         dw = torch.empty_like(w32)
         db = torch.empty(C, device=x.device, dtype=torch.float32) if ctx.has_bias else None
-        rc = _lib.lib().mia_dwconv2d_bwd(x.data_ptr(), w32.data_ptr(), b32.data_ptr() if ctx.has_bias else 0, dy.data_ptr(), dx.data_ptr(),
-                                         dw.data_ptr(), 0 if db is None else db.data_ptr(), B, C, H, W, int(ctx.silu), _DT[x.dtype],
-                                         torch.cuda.current_stream(x.device).cuda_stream)
-        if rc != 0:
-            raise RuntimeError(f"dwconv2d_bwd: {_lib.lib().mia_dwconv2d_last_error().decode()} (code {rc})")
+        _lib.call("mia_dwconv2d_bwd", "dwconv2d_bwd", x.device, x.data_ptr(), w32.data_ptr(), b32.data_ptr() if ctx.has_bias else 0,
+                  dy.data_ptr(), dx.data_ptr(), dw.data_ptr(), 0 if db is None else db.data_ptr(), B, C, H, W, int(ctx.silu),
+                  _lib.dtype_code(x.dtype))
         return dx, dw.view(C, 1, 3, 3).to(ctx.wdtype), (db.to(ctx.bdtype) if db is not None else None), None
 
 
@@ -94,7 +82,7 @@ def cross_scan_fwd(x: torch.Tensor) -> torch.Tensor:
     B, C, H, W = x.shape
     x = x.contiguous()
     xs = x.new_empty((B, 4, C, H * W))
-    _cs_call(_lib.lib().mia_cross_scan, x, xs, B, C, H, W)
+    _cs_call("mia_cross_scan", x, xs, B, C, H, W)
     return xs
 
 
@@ -103,7 +91,7 @@ def cross_merge_fwd(ys: torch.Tensor, H: int, W: int) -> torch.Tensor:
     B, K, C, L = ys.shape
     ys = ys.contiguous()
     y = ys.new_empty((B, C, L))
-    _cs_call(_lib.lib().mia_cross_merge, ys, y, B, C, H, W)
+    _cs_call("mia_cross_merge", ys, y, B, C, H, W)
     return y
 
 

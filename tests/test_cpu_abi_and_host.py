@@ -38,19 +38,103 @@ def test_library_exports_every_declared_symbol():
 
 
 def test_struct_layout_matches_header(tmp_path):
-    from medical_image_analysis_b200._lib import MiaSSParams
-    src = tmp_path / "sz.c"
-    fields = [f for f, _ in MiaSSParams._fields_]
-    lines = "\n".join(f'printf("{f} %zu\\n", offsetof(mia_ss_params, {f}));' for f in fields)
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "mia_selective_scan.h"\nint main(){printf("size %zu\\n", '
-                   'sizeof(mia_ss_params));' + lines + "return 0;}")
-    exe = tmp_path / "sz"
+    """Each ctypes mirror (mia_ss_params, mia_ssu_params, mia_bdl) has the C struct's size and every field at the C offset."""
+    from medical_image_analysis_b200._lib import MiaBdl, MiaSSParams, MiaSSUParams
     cc = "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else "gcc"
-    subprocess.check_call([cc, "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    out = dict(l.split() for l in subprocess.check_output([str(exe)], text=True).splitlines())
-    assert int(out["size"]) == ctypes.sizeof(MiaSSParams)
-    for f in fields:
-        assert int(out[f]) == getattr(MiaSSParams, f).offset, f
+    for mirror, ctype in ((MiaSSParams, "mia_ss_params"), (MiaSSUParams, "mia_ssu_params"), (MiaBdl, "mia_bdl")):
+        src = tmp_path / f"{ctype}.c"
+        fields = [f for f, _ in mirror._fields_]
+        lines = "\n".join(f'printf("{f} %zu\\n", offsetof({ctype}, {f}));' for f in fields)
+        src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "mia_selective_scan.h"\nint main(){printf("size %zu\\n", '
+                       f'sizeof({ctype}));' + lines + "return 0;}")
+        exe = tmp_path / ctype
+        subprocess.check_call([cc, "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
+        out = dict(l.split() for l in subprocess.check_output([str(exe)], text=True).splitlines())
+        assert int(out["size"]) == ctypes.sizeof(mirror), ctype
+        for f in fields:
+            assert int(out[f]) == getattr(mirror, f).offset, (ctype, f)
+
+
+def _header_prototypes():
+    """name -> (parameter types, return type) of every function in the extern "C" blocks of include/*.h."""
+    import glob
+    protos = {}
+    for hdr in sorted(glob.glob(os.path.join(ROOT, "include", "*.h"))):
+        text = re.sub(r"/\*.*?\*/", "", open(hdr).read(), flags=re.S)
+        body = text[text.index('extern "C"'):]
+        for ret, name, params in re.findall(r"([A-Za-z_][\w ]*?\**)\s*\b(mia_\w+)\s*\(([^)]*)\)\s*;", body):
+            params = [] if params.strip() == "void" else [re.sub(r"\s*\w+$", "", p.strip()) if not p.strip().endswith("*") else p.strip()
+                                                          for p in params.split(",")]
+            protos[name] = (params, ret.strip())
+    return protos
+
+
+def _ctype_of(decl):
+    """The ctypes type a C parameter / return type maps to in the binding."""
+    from medical_image_analysis_b200 import _lib
+    decl = " ".join(decl.replace("*", " * ").split())
+    if decl == "const char *":
+        return ctypes.c_char_p
+    structs = {"mia_ss_params": _lib.MiaSSParams, "mia_ssu_params": _lib.MiaSSUParams, "mia_bdl": _lib.MiaBdl}
+    if decl.endswith("*"):
+        base = decl.replace("const", "").replace("*", "").strip()
+        return ctypes.POINTER(structs[base]) if base in structs else ctypes.c_void_p
+    return {"int": ctypes.c_int, "long long": ctypes.c_longlong, "size_t": ctypes.c_size_t, "uint64_t": ctypes.c_uint64}[decl]
+
+
+def test_binding_table_matches_header_prototypes():
+    """_lib.ABI states, for every function include/*.h declares, the argtypes and restype of its prototype (a c_int where the
+    header says long long would truncate silently) and an error getter that the table and the library both have."""
+    from medical_image_analysis_b200 import _lib
+    lib = _lib.lib()
+    protos = _header_prototypes()
+    assert len(protos) >= 30 and "mia_causal_conv1d_bwd_ex" in protos and "mia_gemm" in protos
+    assert set(protos) == set(_lib.ABI), set(protos) ^ set(_lib.ABI)
+    for name, (params, ret) in protos.items():
+        argtypes, restype, getter = _lib.ABI[name]
+        assert [_ctype_of(p) for p in params] == argtypes, name
+        assert _ctype_of(ret) == restype, name
+        assert getattr(lib, name).argtypes == argtypes and getattr(lib, name).restype == restype, name
+        if getter is not None:
+            assert params[-1].endswith("*") and ret == "int", name           # launches: trailing cuda_stream, rc
+            assert _lib.ABI[getter] == ([], ctypes.c_char_p, None), name
+
+
+def test_call_raises_with_the_entry_points_own_channel():
+    """_lib.call reports a failure with the message of the entry point's own error channel, under the caller's prefix; these
+    failures happen before any CUDA call, so device=None (no device, null stream) reaches them."""
+    from medical_image_analysis_b200 import _lib
+    _lib.lib()
+    buf = ctypes.create_string_buffer(64)
+    p = ctypes.cast(buf, ctypes.c_void_p).value
+    with pytest.raises(RuntimeError) as e:
+        _lib.call("mia_dwconv2d_fwd", "dwconv2d_fwd", None, p, p, None, p, 1, 1, 1, 16384, 1, _lib.MIA_F32)
+    assert str(e.value) == ("dwconv2d_fwd: dwconv2d_fwd: a 1 x 16384 float32 plane needs 262224 bytes of shared memory per block, "
+                            "more than the 232448-byte (227 KB) limit (code -1)")
+    ops = (_lib.MiaBdl * 1)(_lib.MiaBdl(p, 0, 0, 1))
+    with pytest.raises(RuntimeError) as e:
+        _lib.call("mia_causal_conv1d_fwd_ex", "causal_conv1d_fwd_ex", None, ctypes.byref(ops[0]), p, None, ops, 1, 0, 4, 8, 4, 1,
+                  _lib.MIA_BF16)
+    assert str(e.value) == "causal_conv1d_fwd_ex: causal_conv1d_fwd_ex: bad sizes (code -1)"
+    with pytest.raises(RuntimeError) as e:                                    # the decode step reports on the scan's channel
+        _lib.call("mia_selective_state_update", "selective_state_update", None, None)
+    assert str(e.value) == "selective_state_update: selective_state_update: null params (code -1)"
+    assert _lib.lib().mia_last_error() == b"selective_state_update: null params"
+    with pytest.raises(RuntimeError) as e:                                    # ... and the decode conv on the conv channel
+        _lib.call("mia_causal_conv1d_update", "causal_conv1d_update", None, None, p, p, None, p, 1, 4, 4, 1, 2, 2, 0, 0,
+                  4, 16, 4, 1, 4, 1, 4)
+    assert str(e.value) == "causal_conv1d_update: causal_conv1d_update: null x / conv_state / weight / out (code -1)"
+    assert _lib.lib().mia_conv_last_error() == b"causal_conv1d_update: null x / conv_state / weight / out"
+
+
+def test_cross_scan_rejects_unknown_dtype_without_gpu():
+    lib = _lib()
+    buf = ctypes.create_string_buffer(64)
+    p = ctypes.cast(buf, ctypes.c_void_p)
+    assert lib.mia_cross_scan(p, p, 1, 1, 2, 2, 7, None) == -1
+    assert lib.mia_cs_last_error() == b"cross scan / merge: dtype must be MIA_F32, MIA_F16 or MIA_BF16"
+    assert lib.mia_silu_gate(p, p, p, 4, 7, 7, None) == -1
+    assert lib.mia_cs_last_error() == b"silu_gate: dtype must be MIA_F32, MIA_F16 or MIA_BF16"
 
 
 def test_chunk_geometry():
