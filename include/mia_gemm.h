@@ -37,6 +37,24 @@ int mia_gemm_tn(const void *A, const void *W, const float *bias, void *C, int M,
  * The wgmma transpose bits select the layout; TMA boxes are [64 k][64 mn] for it. */
 int mia_gemm(const void *A, const void *B, const float *bias, void *C, int M, int N, int K, long long lda, long long ldb, long long ldc,
              int a_mn_major, int b_mn_major, int in_dtype, int out_dtype, int act, void *cuda_stream);
+/* SwiGLU MLP (w3(silu(w1(x)) * w2(x)), models_mamba.py:59-83) around the same kernel.  Hp = H rounded up to a multiple of 64.
+ *
+ * Forward: one GEMM whose B tile pairs W1 and W2 rows: a = x W1^T + b1 and b = x W2^T + b2 accumulate in fp32 in the same
+ * thread, and the epilogue rounds a and b to dtype (bit-identical to two mia_gemm_tn calls with those biases) and writes
+ *   h (M, H, pitch ldh)      round(silu(a) * b), computed from the rounded a and b
+ *   ab (M, 2 Hp, pitch ldab) a in columns [0, H), b in [Hp, Hp + H), pad columns 0; NULL (inference) writes h only.
+ * x (M, K), w1 / w2 (H, K) nn.Linear layout; b1 / b2 fp32 (H) or NULL.
+ *
+ * Backward: g = dy . W3 (dy (M, N_out), W3 (N_out, H) read in place), and from a, b in ab and s = sigmoid(a):
+ *   dab (M, 2 Hp, pitch lddab)  da = g b s (1 + a (1 - s)) in [0, H), db = g a s in [Hp, Hp + H), each rounded once, pads 0
+ *   h (M, H, pitch ldh)         round(a s b), bit-identical to the forward's h, for W3's gradient (NULL: not written).
+ *
+ * dtype is MIA_GEMM_BF16 or MIA_GEMM_F16 for every operand.  Pitches are multiples of 8 elements covering a row (ldab /
+ * lddab >= 2 Hp), pointers 16-byte aligned.  Errors as for mia_gemm_tn. */
+int mia_gemm_swiglu_fwd(const void *x, const void *w1, const void *w2, const float *b1, const float *b2, void *h, void *ab, int M, int H,
+                        int K, long long ldx, long long ldw1, long long ldw2, long long ldh, long long ldab, int dtype, void *cuda_stream);
+int mia_gemm_swiglu_bwd(const void *dy, const void *w3, const void *ab, void *dab, void *h, int M, int H, int N_out, long long lddy,
+                        long long ldw3, long long ldab, long long lddab, long long ldh, int dtype, void *cuda_stream);
 const char *mia_gemm_last_error(void);
 
 #ifdef __cplusplus

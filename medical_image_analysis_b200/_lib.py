@@ -109,6 +109,8 @@ ABI = {
     "mia_causal_conv1d_update": ([_vp] * 5 + [_I] * 8 + [_LL] * 7 + [_vp], _I, _CONV),
     "mia_gemm_tn": ([_vp] * 4 + [_I] * 3 + [_LL] * 3 + [_I] * 3 + [_vp], _I, _GEMM),
     "mia_gemm": ([_vp] * 4 + [_I] * 3 + [_LL] * 3 + [_I] * 5 + [_vp], _I, _GEMM),
+    "mia_gemm_swiglu_fwd": ([_vp] * 7 + [_I] * 3 + [_LL] * 5 + [_I, _vp], _I, _GEMM),
+    "mia_gemm_swiglu_bwd": ([_vp] * 5 + [_I] * 3 + [_LL] * 5 + [_I, _vp], _I, _GEMM),
 }
 
 DTYPE_CODES = {torch.float32: MIA_F32, torch.float16: MIA_F16, torch.bfloat16: MIA_BF16}

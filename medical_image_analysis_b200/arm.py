@@ -6,8 +6,9 @@ constructor arguments, same parameter names and shapes (``A_log``, ``D``, ``conv
 ``_b`` / ``_c`` / ``_c_b`` / ``_d`` / ``_d_b`` direction copies), so the published MambaXray-VL checkpoints load unchanged.
 
 What runs where: every scan is ``selective_scan_fn`` (CUDA, with the z gate), the depth-wise conv + SiLU is the CUDA
-``causal_conv1d_fn``, in_proj / out_proj / SwiGLU / the patch embedding go through the wgmma GEMM for bf16 / fp16
-activations; the four-direction (v3) mixer is one autograd op (MambaV3Fn, the scan orders as index maps in the kernels),
+``causal_conv1d_fn``, in_proj / out_proj / the patch embedding go through the wgmma GEMM for bf16 / fp16 activations, and
+so does the SwiGLU MLP, as one autograd op (SwiGLUFn: w1 and w2 in one GEMM with the gate in its epilogue); the
+four-direction (v3) mixer is one autograd op (MambaV3Fn, the scan orders as index maps in the kernels),
 and the six-direction (v4) orchestration is the reference's, stated once over a table of directions.  Parity: tests/golden/modules_arm.npz holds the outputs of the reference's
 own modules (its fused ops evaluated by its own slow path, see tests/golden/make_golden_modules.py).
 """
@@ -437,8 +438,135 @@ class PatchEmbed(nn.Module):
         return self.norm(x)
 
 
+# ---------------------------------------------------------------------------------------------------------
+# The SwiGLU MLP as one autograd op.  DESIGN.md section 3.14.
+def _pad64(n):
+    return (n + 63) // 64 * 64
+
+
+class SwiGLUFn(torch.autograd.Function):
+    """w3(silu(w1(x)) * w2(x)) (models_mamba.py:59-83 with subln=False) as ONE op on the wgmma GEMM: w1 and w2 run as one
+    GEMM whose tile pairs their rows, so a = w1(x) and b = w2(x) meet in one thread and the epilogue writes the hidden
+    h = silu(a) b (mia_gemm_swiglu_fwd); w3 reads h in place.  The backward's w3 dgrad writes da / db and the recomputed h
+    from its epilogue (mia_gemm_swiglu_bwd); dx and [dW1; dW2] are one GEMM each over the packed (M, 2 Hp) gradient.
+
+    Saved (checkpoint_lvl 0): x in the activation dtype and the packed a / b (M, 2 Hp); level 1 keeps x only and reruns the
+    forward kernel for a / b.  Both give the same bits.  Hp = H rounded up to 64; with nothing to differentiate, nothing is
+    saved and a / b are not written."""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, x, w1, b1, w2, b2, w3, b3, checkpoint_lvl, train):
+        if checkpoint_lvl not in (0, 1):
+            raise ValueError(f"checkpoint_lvl must be 0 or 1, got {checkpoint_lvl!r}")
+        if not x.is_cuda:
+            raise RuntimeError("swiglu_fn: this build has no CPU path (x must be a CUDA tensor)")
+        T = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled() else x.dtype
+        if T not in (torch.bfloat16, torch.float16):
+            raise RuntimeError(f"swiglu_fn: activations must be bfloat16 or float16, directly or under autocast (got {T})")
+        H, K = w1.shape
+        N = w3.shape[0]
+        if tuple(w2.shape) != (H, K) or tuple(w3.shape) != (N, H) or x.shape[-1] != K:
+            raise RuntimeError(f"swiglu_fn: shapes do not chain: x {tuple(x.shape)}, w1 {tuple(w1.shape)}, w2 {tuple(w2.shape)}, w3 {tuple(w3.shape)}")
+        if K % 8 or N % 8:
+            raise RuntimeError(f"swiglu_fn: in_features ({K}) and out_features ({N}) must be multiples of 8")
+        lead = x.shape[:-1]
+        x2 = x.to(T).reshape(-1, K)
+        if not _gemm._mn_ok(x2):
+            x2 = x2.contiguous()
+        M, Hp = x2.shape[0], _pad64(H)
+        if M == 0:
+            raise RuntimeError("swiglu_fn: empty input")
+        ctx.sizes = (M, H, Hp, K, N, T, checkpoint_lvl)
+        ab = torch.empty((M, 2 * Hp), dtype=T, device=x.device) if train else None
+        h = torch.empty((M, Hp), dtype=T, device=x.device)
+        SwiGLUFn._gate(x2, w1, b1, w2, b2, ab, h, ctx)
+        w3p = SwiGLUFn._w3(w3, ctx)
+        y = torch.empty((M, N), dtype=T, device=x.device)
+        b3f = None if b3 is None else b3.detach().float().contiguous()
+        _lib.call("mia_gemm_tn", "swiglu_fn w3", x.device, h.data_ptr(), w3p.data_ptr(), None if b3f is None else b3f.data_ptr(), y.data_ptr(),
+                  M, N, H, h.stride(0), w3p.stride(0), y.stride(0), _lib.dtype_code(T), _lib.dtype_code(T), _gemm.ACT_NONE)
+        if train:
+            ctx.save_for_backward(x2, w1, b1, w2, b2, w3, *([ab] if checkpoint_lvl == 0 else []))
+            ctx.bias_dtypes = tuple(None if b is None else b.dtype for b in (b1, b2, b3))
+        return y.view(*lead, N)
+
+    @staticmethod
+    def _gate(x2, w1, b1, w2, b2, ab, h, ctx):
+        """mia_gemm_swiglu_fwd: h = silu(a) b and, when ab is given, the packed a / b."""
+        M, H, Hp, K, N, T, _ = ctx.sizes
+        w1c, w2c = w1.to(T).contiguous(), w2.to(T).contiguous()
+        b1f, b2f = (None if b is None else b.detach().float().contiguous() for b in (b1, b2))
+        _lib.call("mia_gemm_swiglu_fwd", "swiglu_fn", x2.device, x2.data_ptr(), w1c.data_ptr(), w2c.data_ptr(),
+                  None if b1f is None else b1f.data_ptr(), None if b2f is None else b2f.data_ptr(), h.data_ptr(),
+                  None if ab is None else ab.data_ptr(), M, H, K, x2.stride(0), w1c.stride(0), w2c.stride(0), h.stride(0),
+                  0 if ab is None else ab.stride(0), _lib.dtype_code(T))
+
+    @staticmethod
+    def _w3(w3, ctx):
+        """W3 in the activation dtype with a row pitch that is a multiple of 8 (zero-padded to Hp columns when H is not)."""
+        M, H, Hp, K, N, T, _ = ctx.sizes
+        if H % 8 == 0:
+            return w3.to(T).contiguous()
+        w3p = torch.zeros((N, Hp), dtype=T, device=w3.device)
+        w3p[:, :H] = w3
+        return w3p
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, dy):
+        M, H, Hp, K, N, T, lvl = ctx.sizes
+        x2, w1, b1, w2, b2, w3, *keep = ctx.saved_tensors
+        dev = x2.device
+        need_x, need_w1, need_b1, need_w2, need_b2, need_w3, need_b3 = ctx.needs_input_grad[:7]
+        dy2 = dy.to(T).reshape(M, N)
+        if not _gemm._mn_ok(dy2):
+            dy2 = dy2.contiguous()
+        h = torch.empty((M, Hp), dtype=T, device=dev) if need_w3 or lvl == 1 else None
+        if lvl == 0:
+            ab = keep[0]
+        else:                                                      # rerun the forward kernel: a / b and h, bit for bit
+            ab = torch.empty((M, 2 * Hp), dtype=T, device=dev)
+            SwiGLUFn._gate(x2, w1, b1, w2, b2, ab, h, ctx)
+        w3p = SwiGLUFn._w3(w3, ctx)
+        dab = torch.empty((M, 2 * Hp), dtype=T, device=dev)
+        h_bwd = h if lvl == 0 else None
+        _lib.call("mia_gemm_swiglu_bwd", "swiglu_fn backward", dev, dy2.data_ptr(), w3p.data_ptr(), ab.data_ptr(), dab.data_ptr(),
+                  None if h_bwd is None else h_bwd.data_ptr(), M, H, N, dy2.stride(0), w3p.stride(0), ab.stride(0), dab.stride(0),
+                  Hp if h_bwd is None else h_bwd.stride(0), _lib.dtype_code(T))
+        del ab
+        dx = dw1 = db1 = dw2 = db2 = dw3 = db3 = None
+        if need_w3:                                                # dW3 = dy^T h
+            dw3 = _gemm.gemm(dy2, h[:, :H], True, True, torch.float32).to(w3.dtype)
+        del h
+        if need_b3:
+            db3 = dy2.sum(0, dtype=torch.float32).to(ctx.bias_dtypes[2])
+        if need_x:                                                 # dx = [da, db] . [W1; W2], K = 2 Hp over a zero-padded stack
+            wst = torch.zeros((2 * Hp, K), dtype=T, device=dev)
+            wst[:H] = w1
+            wst[Hp:Hp + H] = w2
+            dx = _gemm.gemm(dab, wst, False, True).view(*dy.shape[:-1], K)
+        if need_w1 or need_w2:                                     # [dW1; dW2] = [da, db]^T x
+            dw12 = _gemm.gemm(dab, x2, True, True, torch.float32)
+            dw1, dw2 = dw12[:H].to(w1.dtype), dw12[Hp:Hp + H].to(w2.dtype)
+        if need_b1 or need_b2:
+            db12 = dab.sum(0, dtype=torch.float32)
+            db1 = None if b1 is None else db12[:H].to(ctx.bias_dtypes[0])
+            db2 = None if b2 is None else db12[Hp:Hp + H].to(ctx.bias_dtypes[1])
+        return dx, dw1, db1, dw2, db2, dw3, db3, None, None
+
+
+def swiglu_fn(x, w1, b1, w2, b2, w3, b3, checkpoint_lvl=0):
+    """w3(silu(w1(x)) * w2(x)) for bf16 / fp16 CUDA activations (directly or under autocast) as one op: x (..., in), w1 / w2
+    (H, in), w3 (out, H) with in and out multiples of 8 (any H), biases (H) / (out) or None.  checkpoint_lvl 0 (default) keeps
+    the packed w1(x) / w2(x) for the backward, 1 recomputes them; both give the same bits."""
+    train = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, w1, b1, w2, b2, w3, b3))
+    return SwiGLUFn.apply(x, w1, b1, w2, b2, w3, b3, checkpoint_lvl, train)
+
+
 class SwiGLU(nn.Module):
-    """models_mamba.py:59-83."""
+    """models_mamba.py:59-83.  For bf16 / fp16 CUDA activations with the SiLU act and no sub-LN (what Block builds) the
+    layer runs as one op (swiglu_fn); every other configuration runs the composition, _forward_composed."""
 
     def __init__(self, in_features, hidden_features=None, out_features=None, act_layer=nn.SiLU, drop=0.0, norm_layer=nn.LayerNorm, subln=False):
         super().__init__()
@@ -450,7 +578,17 @@ class SwiGLU(nn.Module):
         self.w3 = nn.Linear(hidden_features, out_features)
         self.drop = nn.Dropout(drop)
 
+    def _fused_ok(self, x):
+        T = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled() and x.is_cuda else x.dtype
+        return (x.is_cuda and T in (torch.bfloat16, torch.float16) and type(self.act) is nn.SiLU and isinstance(self.ffn_ln, nn.Identity)
+                and x.numel() > 0 and self.w1.in_features % 8 == 0 and self.w3.out_features % 8 == 0)
+
     def forward(self, x):
+        if self._fused_ok(x):
+            return self.drop(swiglu_fn(x, self.w1.weight, self.w1.bias, self.w2.weight, self.w2.bias, self.w3.weight, self.w3.bias))
+        return self._forward_composed(x)
+
+    def _forward_composed(self, x):
         hidden = self.act(_gemm.linear(x, self.w1.weight, self.w1.bias)) * _gemm.linear(x, self.w2.weight, self.w2.bias)
         return self.drop(_gemm.linear(self.ffn_ln(hidden), self.w3.weight, self.w3.bias))
 

@@ -20,6 +20,7 @@
 //                 8-column group; the producer already streams the next tile's stages meanwhile.
 // Out-of-range rows / columns / K tail are zero-filled by TMA and masked in the epilogue, so any M, N and any K with
 // K % 8 == 0 (16-byte rows) work.  No split-K: K is at most 16384 (patch-embed conv4/4) and M is large on this path.
+// The SwiGLU MLP (models_mamba.py:59-83) runs on the same CTA with a paired-B tile and its own epilogues (kEpiSwiglu*).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -43,6 +44,23 @@ struct GemmArgs {
     void *C;
     long long ldc;
     int num_m_blocks, num_n_blocks, num_k_blocks;
+};
+
+// Epilogue of a tile.  kEpiLinear: act(acc + bias) into C (mia_gemm_tn / mia_gemm).  The SwiGLU pair (mia_gemm_swiglu_*):
+//   kEpiSwigluFwd  paired B tile: columns [0, BN/2) of the tile are x.W1^T, [BN/2, BN) x.W2^T at the same hidden columns;
+//                  a = round(acc1 + b1), b = round(acc2 + b2) -> ab (optional), h = round(silu(a) b)
+//   kEpiSwigluBwd  acc = g = dy.W3 (W3 read MN-major); a, b loaded from ab at the fragment's own (row, col) ->
+//                  dab = (round(g b s (1 + a (1 - s))), round(g a s)), h = round(a s b) (optional), s = sigmoid(a)
+// ab / dab are (M, 2 Hp): the a / da half in columns [0, H), the b / db half in [Hp, Hp + H), pad columns written as 0.
+enum { kEpiLinear = 0, kEpiSwigluFwd = 1, kEpiSwigluBwd = 2 };
+
+struct SwigluArgs {
+    const float *b1, *b2;      // fwd biases (fp32, may be NULL)
+    void *h;                   // (M, H), pitch ldh (bwd: may be NULL)
+    void *ab;                  // fwd: output, may be NULL; bwd: input
+    void *dab;                 // bwd output
+    long long ldh, ldab, lddab;
+    int H, Hp;
 };
 
 __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *tm, int c0, int c1, uint64_t *bar) {
@@ -138,9 +156,71 @@ __device__ __forceinline__ void store_pair(const GemmArgs &g, int row, int col, 
     }
 }
 
+template <bool kF16>
+__device__ __forceinline__ float round_to(float v) {
+    return kF16 ? __half2float(__float2half_rn(v)) : __bfloat162float(__float2bfloat16_rn(v));
+}
+template <bool kF16>
+__device__ __forceinline__ float2 load2(const void *base, long long ld, int row, int col) {
+    const uint32_t w = *reinterpret_cast<const uint32_t *>(reinterpret_cast<const uint16_t *>(base) + (size_t)row * ld + col);
+    if (kF16) return __half22float2(*reinterpret_cast<const __half2 *>(&w));
+    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&w));
+}
+// two adjacent 16-bit elements of a row; `both` false stores the first only
+template <bool kF16>
+__device__ __forceinline__ void store2(void *base, long long ld, int row, int col, float v0, float v1, bool both) {
+    uint16_t *dst = reinterpret_cast<uint16_t *>(base) + (size_t)row * ld + col;
+    uint32_t w;
+    if (kF16) { __half2 h = __floats2half2_rn(v0, v1); w = *reinterpret_cast<uint32_t *>(&h); }
+    else { __nv_bfloat162 h = __floats2bfloat162_rn(v0, v1); w = *reinterpret_cast<uint32_t *>(&h); }
+    if (both) *reinterpret_cast<uint32_t *>(dst) = w;
+    else dst[0] = (uint16_t)(w & 0xffffu);
+}
+
+// SwiGLU epilogues of one thread's fragment (see kEpiSwigluFwd / kEpiSwigluBwd).  Host checks make every pitch even and
+// every base 16-byte aligned, so the pair stores are aligned; Hp is a multiple of 64, so a pair never straddles it.
+// Both compute h as (a s) b from the rounded a and b, so the backward's recomputed h is the forward's, bit for bit.
+__device__ __forceinline__ float sigmoid(float a) { return 1.f / (1.f + __expf(-a)); }
+template <bool kF16>
+__device__ __forceinline__ void swiglu_fwd_pair(const SwigluArgs &sw, int row, int col, float acc_a0, float acc_a1, float acc_b0,
+                                                float acc_b1, float ba0, float ba1, float bb0, float bb1) {
+    const bool in0 = col < sw.H, in1 = col + 1 < sw.H;
+    const float a0 = in0 ? round_to<kF16>(acc_a0 + ba0) : 0.f, a1 = in1 ? round_to<kF16>(acc_a1 + ba1) : 0.f;
+    const float b0 = in0 ? round_to<kF16>(acc_b0 + bb0) : 0.f, b1 = in1 ? round_to<kF16>(acc_b1 + bb1) : 0.f;
+    if (sw.ab) {
+        store2<kF16>(sw.ab, sw.ldab, row, col, a0, a1, true);
+        store2<kF16>(sw.ab, sw.ldab, row, sw.Hp + col, b0, b1, true);
+    }
+    if (in0) store2<kF16>(sw.h, sw.ldh, row, col, a0 * sigmoid(a0) * b0, a1 * sigmoid(a1) * b1, in1);
+}
+
+// silu'(a) / s = 1 + a (1 - s).  It has a root at a = -1.2785: around it fp32 cancels to a relative error above half an
+// fp16 ulp, so where |factor| < 2^-8 (a few representable a) it is recomputed in fp64.
+__device__ __noinline__ float dsilu_factor_f64(float a) {
+    const double e = exp(-(double)a);
+    return (float)(1.0 + (double)a * e / (1.0 + e));
+}
+__device__ __forceinline__ float dsilu_factor(float a, float s) {
+    const float f = 1.f + a * (1.f - s);
+    return fabsf(f) < 0.00390625f ? dsilu_factor_f64(a) : f;
+}
+
+template <bool kF16>
+__device__ __forceinline__ void swiglu_bwd_pair(const SwigluArgs &sw, int row, int col, float g0, float g1) {
+    const bool in0 = col < sw.H, in1 = col + 1 < sw.H;
+    const float2 a = load2<kF16>(sw.ab, sw.ldab, row, col), b = load2<kF16>(sw.ab, sw.ldab, row, sw.Hp + col);
+    const float s0 = sigmoid(a.x), s1 = sigmoid(a.y);
+    const float da0 = in0 ? g0 * b.x * s0 * dsilu_factor(a.x, s0) : 0.f, da1 = in1 ? g1 * b.y * s1 * dsilu_factor(a.y, s1) : 0.f;
+    const float db0 = in0 ? g0 * a.x * s0 : 0.f, db1 = in1 ? g1 * a.y * s1 : 0.f;
+    store2<kF16>(sw.dab, sw.lddab, row, col, da0, da1, true);
+    store2<kF16>(sw.dab, sw.lddab, row, sw.Hp + col, db0, db1, true);
+    if (sw.h && in0) store2<kF16>(sw.h, sw.ldh, row, col, a.x * s0 * b.x, a.y * s1 * b.y, in1);
+}
+
 // The two consumer warpgroups: `cw` (0 / 1) owns rows [64 cw, 64 cw + 64) of every tile of this CTA.
-template <int BN, int kStages, bool kAMN, bool kBMN, bool kF16>
-__device__ __forceinline__ void gemm_consumer(const GemmArgs &g, char *tiles, uint64_t *full, uint64_t *empty, int cw) {
+template <int BN, int kStages, bool kAMN, bool kBMN, bool kF16, int kEpi = kEpiLinear>
+__device__ __forceinline__ void gemm_consumer(const GemmArgs &g, char *tiles, uint64_t *full, uint64_t *empty, int cw,
+                                              const SwigluArgs *sw = nullptr) {
     constexpr int kABytes = kBM * kBK * 2, kStageBytes = kABytes + BN * kBK * 2;
     constexpr int kUnit = BN >= 128 ? 128 : 64;          // columns per wgmma instruction
     const int t = threadIdx.x & 127, lane = t & 31;
@@ -180,19 +260,55 @@ __device__ __forceinline__ void gemm_consumer(const GemmArgs &g, char *tiles, ui
         if (t == 0) mia::mbar_arrive(empty + prev);
 
         const int row0 = mb * kBM + cw * 64 + (t >> 5) * 16 + (lane >> 2);
+        if constexpr (kEpi == kEpiSwigluFwd) {
+            // d[0] holds x.W1^T and d[1] x.W2^T at the same (row, hidden column): the gate needs no data exchange
+            static_assert(BN == 256 && !kBMN, "the paired-B tile is 2 x 128 K-major rows");
 #pragma unroll
-        for (int u = 0; u < BN / kUnit; ++u) {
-#pragma unroll
-            for (int j = 0; j < kUnit / 8; ++j) {
-                const int col = nb * BN + u * kUnit + 8 * j + 2 * (lane & 3);
-                if (col < g.N) {
-                    const float b0 = g.has_bias ? __ldg(g.bias + col) : 0.f;
-                    const float b1 = (g.has_bias && col + 1 < g.N) ? __ldg(g.bias + col + 1) : 0.f;
+            for (int j = 0; j < 16; ++j) {
+                const int col = nb * 128 + 8 * j + 2 * (lane & 3);
+                if (col < sw->Hp) {
+                    const bool in0 = col < sw->H, in1 = col + 1 < sw->H;
+                    const float ba0 = sw->b1 && in0 ? __ldg(sw->b1 + col) : 0.f, ba1 = sw->b1 && in1 ? __ldg(sw->b1 + col + 1) : 0.f;
+                    const float bb0 = sw->b2 && in0 ? __ldg(sw->b2 + col) : 0.f, bb1 = sw->b2 && in1 ? __ldg(sw->b2 + col + 1) : 0.f;
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const int row = row0 + 8 * h;
                         if (row < g.M)
-                            store_pair<kF16>(g, row, col, act_apply(d[u][4 * j + 2 * h] + b0, g.act), act_apply(d[u][4 * j + 2 * h + 1] + b1, g.act));
+                            swiglu_fwd_pair<kF16>(*sw, row, col, d[0][4 * j + 2 * h], d[0][4 * j + 2 * h + 1], d[1][4 * j + 2 * h],
+                                                  d[1][4 * j + 2 * h + 1], ba0, ba1, bb0, bb1);
+                    }
+                }
+            }
+        } else if constexpr (kEpi == kEpiSwigluBwd) {
+#pragma unroll
+            for (int u = 0; u < BN / kUnit; ++u) {
+#pragma unroll
+                for (int j = 0; j < kUnit / 8; ++j) {
+                    const int col = nb * BN + u * kUnit + 8 * j + 2 * (lane & 3);
+                    if (col < sw->Hp) {
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int row = row0 + 8 * h;
+                            if (row < g.M) swiglu_bwd_pair<kF16>(*sw, row, col, d[u][4 * j + 2 * h], d[u][4 * j + 2 * h + 1]);
+                        }
+                    }
+                }
+            }
+        } else {
+#pragma unroll
+            for (int u = 0; u < BN / kUnit; ++u) {
+#pragma unroll
+                for (int j = 0; j < kUnit / 8; ++j) {
+                    const int col = nb * BN + u * kUnit + 8 * j + 2 * (lane & 3);
+                    if (col < g.N) {
+                        const float b0 = g.has_bias ? __ldg(g.bias + col) : 0.f;
+                        const float b1 = (g.has_bias && col + 1 < g.N) ? __ldg(g.bias + col + 1) : 0.f;
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int row = row0 + 8 * h;
+                            if (row < g.M)
+                                store_pair<kF16>(g, row, col, act_apply(d[u][4 * j + 2 * h] + b0, g.act), act_apply(d[u][4 * j + 2 * h + 1] + b1, g.act));
+                        }
                     }
                 }
             }
@@ -200,9 +316,11 @@ __device__ __forceinline__ void gemm_consumer(const GemmArgs &g, char *tiles, ui
     }
 }
 
-template <int BN, int kStages, bool kAMN, bool kBMN, bool kF16>
-__global__ void __launch_bounds__(kGemmThreads, 1) gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                                                                  const GemmArgs g) {
+// The whole CTA: barrier setup, the producer warpgroup and the two consumers.  kEpiSwigluFwd pairs the B tile: W1 rows
+// [n0, n0 + 128) from tmB into its first half and W2's from tmB2 into its second, n0 = 128 nb (tmB2 is unused otherwise).
+template <int BN, int kStages, bool kAMN, bool kBMN, bool kF16, int kEpi>
+__device__ __forceinline__ void gemm_cta(const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmB2, const GemmArgs &g,
+                                         const SwigluArgs *sw) {
     extern __shared__ char smem_raw[];
     // SWIZZLE_128B tiles must sit on 1024-byte boundaries
     char *tiles = reinterpret_cast<char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -238,7 +356,10 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tn_kernel(const __grid_c
                     } else {
                         tma_load_2d(sa, &tmA, kb * kBK, mb * kBM, full + s);
                     }
-                    if (kBMN) {
+                    if constexpr (kEpi == kEpiSwigluFwd) {
+                        tma_load_2d(sb, &tmB, kb * kBK, nb * (BN / 2), full + s);
+                        tma_load_2d(sb + (BN / 2) * kBK * 2, &tmB2, kb * kBK, nb * (BN / 2), full + s);
+                    } else if (kBMN) {
 #pragma unroll
                         for (int i = 0; i < BN / 64; ++i) tma_load_2d(sb + i * 8192, &tmB, nb * BN + 64 * i, kb * kBK, full + s);
                     } else {
@@ -250,8 +371,22 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tn_kernel(const __grid_c
         }
     } else {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-        gemm_consumer<BN, kStages, kAMN, kBMN, kF16>(g, tiles, full, empty, wg - 1);
+        gemm_consumer<BN, kStages, kAMN, kBMN, kF16, kEpi>(g, tiles, full, empty, wg - 1, sw);
     }
+}
+
+template <int BN, int kStages, bool kAMN, bool kBMN, bool kF16>
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                                                                  const GemmArgs g) {
+    gemm_cta<BN, kStages, kAMN, kBMN, kF16, kEpiLinear>(tmA, tmB, tmB, g, nullptr);
+}
+
+// SwiGLU forward (kEpiSwigluFwd: A = x, tmB / tmB2 = W1 / W2, K-major) and backward (kEpiSwigluBwd: A = dy, tmB = W3 read
+// MN-major, tmB2 unused).
+template <int kEpi, int BN, int kStages, bool kBMN, bool kF16>
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_swiglu_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                                                                      const __grid_constant__ CUtensorMap tmB2, const GemmArgs g, const SwigluArgs sw) {
+    gemm_cta<BN, kStages, false, kBMN, kF16, kEpi>(tmA, tmB, tmB2, g, &sw);
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------
@@ -306,6 +441,26 @@ int launch_gemm(const CUtensorMap &tmA, const CUtensorMap &tmB, GemmArgs &g, int
     return mia::launched(mia::kErrGemm, "gemm launch");
 }
 
+// g.N is the hidden width H; a paired-B tile (forward) spans BN / 2 hidden columns, a backward tile BN.
+template <int kEpi, int BN, int kStages, bool kBMN, bool kF16>
+int launch_swiglu(const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmB2, GemmArgs &g, const SwigluArgs &sw, int sms,
+                  cudaStream_t stream) {
+    constexpr int smem = kStages * (kBM * kBK * 2 + BN * kBK * 2) + 2 * kStages * 8 + 1024;
+    constexpr int span = kEpi == kEpiSwigluFwd ? BN / 2 : BN;
+    auto k = &gemm_swiglu_kernel<kEpi, BN, kStages, kBMN, kF16>;
+    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "cudaFuncSetAttribute(gemm_swiglu, %d B): %s", smem, cudaGetErrorString(cudaGetLastError()));
+    g.num_m_blocks = (g.M + kBM - 1) / kBM;
+    g.num_n_blocks = (g.N + span - 1) / span;
+    g.num_k_blocks = (g.K + kBK - 1) / kBK;
+    const int tiles = g.num_m_blocks * g.num_n_blocks;
+    const int grid = tiles < sms ? tiles : sms;
+    k<<<grid, kGemmThreads, smem, stream>>>(tmA, tmB, tmB2, g, sw);
+    return mia::launched(mia::kErrGemm, "gemm_swiglu launch");
+}
+
+long long swiglu_pad(int H) { return ((long long)H + 63) / 64 * 64; }
+
 }  // namespace
 
 static int gemm_impl(const void *A, const void *W, const float *bias, void *C, int M, int N, int K, long long lda, long long ldw, long long ldc,
@@ -358,6 +513,73 @@ int mia_gemm_tn(const void *A, const void *W, const float *bias, void *C, int M,
 int mia_gemm(const void *A, const void *B, const float *bias, void *C, int M, int N, int K, long long lda, long long ldb, long long ldc,
              int a_mn_major, int b_mn_major, int in_dtype, int out_dtype, int act, void *cuda_stream) {
     return gemm_impl(A, B, bias, C, M, N, K, lda, ldb, ldc, a_mn_major != 0, b_mn_major != 0, in_dtype, out_dtype, act, cuda_stream);
+}
+
+int mia_gemm_swiglu_fwd(const void *x, const void *w1, const void *w2, const float *b1, const float *b2, void *h, void *ab, int M, int H,
+                        int K, long long ldx, long long ldw1, long long ldw2, long long ldh, long long ldab, int dtype, void *cuda_stream) {
+    if (!x || !w1 || !w2 || !h) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_fwd: null pointer (x, w1, w2 and h are required)");
+    if (M <= 0 || H <= 0 || K <= 0) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_fwd: empty or negative size (M %d, H %d, K %d)", M, H, K);
+    if (dtype != MIA_GEMM_BF16 && dtype != MIA_GEMM_F16) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_fwd: dtype must be bf16 or fp16");
+    if ((ldx | ldw1 | ldw2 | ldh) % 8 || ldx < K || ldw1 < K || ldw2 < K || ldh < H)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_fwd: row pitches must cover a row and be multiples of 8 elements "
+                         "(ldx %lld, ldw1 %lld, ldw2 %lld, ldh %lld, H %d, K %d)", ldx, ldw1, ldw2, ldh, H, K);
+    const long long Hp = swiglu_pad(H);
+    if (ab && (ldab % 8 || ldab < 2 * Hp))
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_fwd: ldab must be a multiple of 8 and at least 2 Hp = %lld (ldab %lld)", 2 * Hp, ldab);
+    if (((uintptr_t)x | (uintptr_t)w1 | (uintptr_t)w2 | (uintptr_t)h | (uintptr_t)ab) & 15)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_fwd: x, w1, w2, h and ab must be 16-byte aligned");
+    mia::DeviceInfo di;
+    if (mia::device_info(mia::kErrGemm, di) != MIA_OK) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "gemm_swiglu_fwd: cannot query the device");
+    GemmArgs g;
+    memset(&g, 0, sizeof(g));
+    g.M = M; g.N = H; g.K = K; g.in_f16 = dtype == MIA_GEMM_F16;
+    SwigluArgs sw;
+    memset(&sw, 0, sizeof(sw));
+    sw.b1 = b1; sw.b2 = b2; sw.h = h; sw.ab = ab; sw.ldh = ldh; sw.ldab = ldab; sw.H = H; sw.Hp = (int)Hp;
+    CUtensorMap tmA, tmB, tmB2;
+    if (int rc = make_map(&tmA, x, M, K, ldx, kBM, dtype)) return rc;
+    if (int rc = make_map(&tmB, w1, H, K, ldw1, 128, dtype)) return rc;
+    if (int rc = make_map(&tmB2, w2, H, K, ldw2, 128, dtype)) return rc;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    if (g.in_f16) return launch_swiglu<kEpiSwigluFwd, 256, 4, false, true>(tmA, tmB, tmB2, g, sw, di.sms, stream);
+    return launch_swiglu<kEpiSwigluFwd, 256, 4, false, false>(tmA, tmB, tmB2, g, sw, di.sms, stream);
+}
+
+int mia_gemm_swiglu_bwd(const void *dy, const void *w3, const void *ab, void *dab, void *h, int M, int H, int N_out, long long lddy,
+                        long long ldw3, long long ldab, long long lddab, long long ldh, int dtype, void *cuda_stream) {
+    if (!dy || !w3 || !ab || !dab) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_bwd: null pointer (dy, w3, ab and dab are required)");
+    if (M <= 0 || H <= 0 || N_out <= 0)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_bwd: empty or negative size (M %d, H %d, N_out %d)", M, H, N_out);
+    if (dtype != MIA_GEMM_BF16 && dtype != MIA_GEMM_F16) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_bwd: dtype must be bf16 or fp16");
+    if ((lddy | ldw3) % 8 || (h && ldh % 8) || lddy < N_out || ldw3 < H || (h && ldh < H))
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_bwd: row pitches must cover a row and be multiples of 8 elements "
+                         "(lddy %lld, ldw3 %lld, ldh %lld, H %d, N_out %d)", lddy, ldw3, ldh, H, N_out);
+    const long long Hp = swiglu_pad(H);
+    if ((ldab | lddab) % 8 || ldab < 2 * Hp || lddab < 2 * Hp)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_bwd: ldab and lddab must be multiples of 8 and at least 2 Hp = %lld "
+                         "(ldab %lld, lddab %lld)", 2 * Hp, ldab, lddab);
+    if (((uintptr_t)dy | (uintptr_t)w3 | (uintptr_t)ab | (uintptr_t)dab | (uintptr_t)h) & 15)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_swiglu_bwd: dy, w3, ab, dab and h must be 16-byte aligned");
+    mia::DeviceInfo di;
+    if (mia::device_info(mia::kErrGemm, di) != MIA_OK) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "gemm_swiglu_bwd: cannot query the device");
+    GemmArgs g;
+    memset(&g, 0, sizeof(g));
+    g.M = M; g.N = H; g.K = N_out; g.in_f16 = dtype == MIA_GEMM_F16;
+    SwigluArgs sw;
+    memset(&sw, 0, sizeof(sw));
+    sw.h = h; sw.ab = const_cast<void *>(ab); sw.dab = dab; sw.ldh = ldh; sw.ldab = ldab; sw.lddab = lddab; sw.H = H; sw.Hp = (int)Hp;
+    // g = dy . W3: dy [M][N_out] K-major; W3 [N_out][H] read MN-major (rows = k), as LinearTC's dgrad reads it
+    CUtensorMap tmA, tmB;
+    if (int rc = make_map(&tmA, dy, M, N_out, lddy, kBM, dtype)) return rc;
+    if (int rc = make_map(&tmB, w3, N_out, H, ldw3, kBK, dtype)) return rc;
+    const bool wide = (long long)((M + 127) / 128) * ((H + 255) / 256) >= di.sms;      // gemm_impl's choice between 128 and 256
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    if (g.in_f16) {
+        if (wide) return launch_swiglu<kEpiSwigluBwd, 256, 4, true, true>(tmA, tmB, tmB, g, sw, di.sms, stream);
+        return launch_swiglu<kEpiSwigluBwd, 128, 6, true, true>(tmA, tmB, tmB, g, sw, di.sms, stream);
+    }
+    if (wide) return launch_swiglu<kEpiSwigluBwd, 256, 4, true, false>(tmA, tmB, tmB, g, sw, di.sms, stream);
+    return launch_swiglu<kEpiSwigluBwd, 128, 6, true, false>(tmA, tmB, tmB, g, sw, di.sms, stream);
 }
 
 }  // extern "C"
