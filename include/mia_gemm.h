@@ -55,6 +55,24 @@ int mia_gemm_swiglu_fwd(const void *x, const void *w1, const void *w2, const flo
                         int K, long long ldx, long long ldw1, long long ldw2, long long ldh, long long ldab, int dtype, void *cuda_stream);
 int mia_gemm_swiglu_bwd(const void *dy, const void *w3, const void *ab, void *dab, void *h, int M, int H, int N_out, long long lddy,
                         long long ldw3, long long ldab, long long lddab, long long ldh, int dtype, void *cuda_stream);
+/* GELU MLP (fc2(gelu(fc1(x))), vmamba.py:495-514 and timm's Mlp) around the same kernel.  Hp = H rounded up to a multiple of 8.
+ *
+ * Forward: fc1 as one GEMM, x (M, K), w1 (H, K) nn.Linear layout, b1 fp32 (H) or NULL.  The epilogue writes
+ *   pre (M, H, pitch ldpre)  round(x W1^T + b1), bit-identical to mia_gemm_tn(x, w1, b1) (same k order, fp32 bias add)
+ *   h (M, H, pitch ldh)      round(0.5 p (1 + erf(p / sqrt 2))) in fp32 from the rounded p = pre: F.gelu(pre)
+ * and 0 in columns [H, Hp) of both; pre NULL (inference) writes h only.
+ *
+ * Backward: g = dy . W2 in fp32, never rounded (dy (M, N_out), W2 (N_out, H) read in place), and from p in pre:
+ *   dpre (M, H, pitch lddpre)  round(g (Phi(p) + p phi(p))), Phi from erfc, recomputed in fp64 where the factor is below
+ *                              2^-8 (around its root at p = -0.7518); 0 in columns [H, Hp)
+ *   h (M, H, pitch ldh)        the forward's expression, bit-identical to its h, for W2's gradient (NULL: not written).
+ *
+ * dtype is MIA_GEMM_BF16 or MIA_GEMM_F16 for every operand.  Pitches are multiples of 8 elements covering a row (so
+ * ldpre, lddpre, ldh >= Hp), pointers 16-byte aligned.  Errors as for mia_gemm_tn. */
+int mia_gemm_gelu_fwd(const void *x, const void *w1, const float *b1, void *h, void *pre, int M, int H, int K, long long ldx, long long ldw1,
+                      long long ldh, long long ldpre, int dtype, void *cuda_stream);
+int mia_gemm_gelu_bwd(const void *dy, const void *w2, const void *pre, void *dpre, void *h, int M, int H, int N_out, long long lddy,
+                      long long ldw2, long long ldpre, long long lddpre, long long ldh, int dtype, void *cuda_stream);
 const char *mia_gemm_last_error(void);
 
 #ifdef __cplusplus

@@ -111,6 +111,8 @@ ABI = {
     "mia_gemm": ([_vp] * 4 + [_I] * 3 + [_LL] * 3 + [_I] * 5 + [_vp], _I, _GEMM),
     "mia_gemm_swiglu_fwd": ([_vp] * 7 + [_I] * 3 + [_LL] * 5 + [_I, _vp], _I, _GEMM),
     "mia_gemm_swiglu_bwd": ([_vp] * 5 + [_I] * 3 + [_LL] * 5 + [_I, _vp], _I, _GEMM),
+    "mia_gemm_gelu_fwd": ([_vp] * 5 + [_I] * 3 + [_LL] * 4 + [_I, _vp], _I, _GEMM),
+    "mia_gemm_gelu_bwd": ([_vp] * 5 + [_I] * 3 + [_LL] * 5 + [_I, _vp], _I, _GEMM),
 }
 
 DTYPE_CODES = {torch.float32: MIA_F32, torch.float16: MIA_F16, torch.bfloat16: MIA_BF16}

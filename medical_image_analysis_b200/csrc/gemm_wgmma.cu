@@ -20,7 +20,8 @@
 //                 8-column group; the producer already streams the next tile's stages meanwhile.
 // Out-of-range rows / columns / K tail are zero-filled by TMA and masked in the epilogue, so any M, N and any K with
 // K % 8 == 0 (16-byte rows) work.  No split-K: K is at most 16384 (patch-embed conv4/4) and M is large on this path.
-// The SwiGLU MLP (models_mamba.py:59-83) runs on the same CTA with a paired-B tile and its own epilogues (kEpiSwiglu*).
+// The SwiGLU MLP (models_mamba.py:59-83) runs on the same CTA with a paired-B tile and its own epilogues (kEpiSwiglu*);
+// the GELU MLP's fc1 and fc2-dgrad (vmamba.py:495-514, timm Mlp) run on it with the GELU and its derivative in theirs (kEpiGelu*).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -52,13 +53,19 @@ struct GemmArgs {
 //   kEpiSwigluBwd  acc = g = dy.W3 (W3 read MN-major); a, b loaded from ab at the fragment's own (row, col) ->
 //                  dab = (round(g b s (1 + a (1 - s))), round(g a s)), h = round(a s b) (optional), s = sigmoid(a)
 // ab / dab are (M, 2 Hp): the a / da half in columns [0, H), the b / db half in [Hp, Hp + H), pad columns written as 0.
-enum { kEpiLinear = 0, kEpiSwigluFwd = 1, kEpiSwigluBwd = 2 };
+// The GELU pair (mia_gemm_gelu_*), Hp = H rounded up to 8:
+//   kEpiGeluFwd    acc = x.W1^T: p = round(acc + b1) -> ab = pre (optional), h = round(gelu(p))
+//   kEpiGeluBwd    acc = g = dy.W2 (W2 read MN-major); p loaded from ab = pre at the fragment's own (row, col) ->
+//                  dab = dpre = round(g gelu'(p)), h = round(gelu(p)) (optional)
+// pre / dpre / h are (M, Hp) with columns [H, Hp) written as 0.
+enum { kEpiLinear = 0, kEpiSwigluFwd = 1, kEpiSwigluBwd = 2, kEpiGeluFwd = 3, kEpiGeluBwd = 4 };
 
-struct SwigluArgs {
-    const float *b1, *b2;      // fwd biases (fp32, may be NULL)
+// Operands of the fused epilogues (every mode but kEpiLinear).
+struct EpiArgs {
+    const float *b1, *b2;      // fwd biases (fp32, may be NULL; b2: SwiGLU only)
     void *h;                   // (M, H), pitch ldh (bwd: may be NULL)
-    void *ab;                  // fwd: output, may be NULL; bwd: input
-    void *dab;                 // bwd output
+    void *ab;                  // saved pre-activations (SwiGLU: packed a / b; GELU: pre).  fwd: output, may be NULL; bwd: input
+    void *dab;                 // bwd output: their gradients, in ab's layout
     long long ldh, ldab, lddab;
     int H, Hp;
 };
@@ -127,10 +134,14 @@ __device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(uint32_t smem_addr) {
     return (uint64_t)((smem_addr & 0x3ffffu) >> 4) | ((uint64_t)(8192 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 
+// The operation order of ATen's CUDA GELU (x 0.5 (1 + erf(x sqrt(1/2))) in fp32), so that a GELU epilogue on a rounded
+// pre-activation writes what F.gelu writes for it.
+__device__ __forceinline__ float gelu(float p) { return 0.5f * p * (1.f + erff(p * 0.70710678118654752f)); }
+
 __device__ __forceinline__ float act_apply(float v, int act) {
     switch (act) {
         case MIA_ACT_RELU: return fmaxf(v, 0.f);
-        case MIA_ACT_GELU: return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
+        case MIA_ACT_GELU: return gelu(v);
         case MIA_ACT_SILU: return v / (1.f + __expf(-v));
         default: return v;
     }
@@ -182,7 +193,7 @@ __device__ __forceinline__ void store2(void *base, long long ld, int row, int co
 // Both compute h as (a s) b from the rounded a and b, so the backward's recomputed h is the forward's, bit for bit.
 __device__ __forceinline__ float sigmoid(float a) { return 1.f / (1.f + __expf(-a)); }
 template <bool kF16>
-__device__ __forceinline__ void swiglu_fwd_pair(const SwigluArgs &sw, int row, int col, float acc_a0, float acc_a1, float acc_b0,
+__device__ __forceinline__ void swiglu_fwd_pair(const EpiArgs &sw, int row, int col, float acc_a0, float acc_a1, float acc_b0,
                                                 float acc_b1, float ba0, float ba1, float bb0, float bb1) {
     const bool in0 = col < sw.H, in1 = col + 1 < sw.H;
     const float a0 = in0 ? round_to<kF16>(acc_a0 + ba0) : 0.f, a1 = in1 ? round_to<kF16>(acc_a1 + ba1) : 0.f;
@@ -206,7 +217,7 @@ __device__ __forceinline__ float dsilu_factor(float a, float s) {
 }
 
 template <bool kF16>
-__device__ __forceinline__ void swiglu_bwd_pair(const SwigluArgs &sw, int row, int col, float g0, float g1) {
+__device__ __forceinline__ void swiglu_bwd_pair(const EpiArgs &sw, int row, int col, float g0, float g1) {
     const bool in0 = col < sw.H, in1 = col + 1 < sw.H;
     const float2 a = load2<kF16>(sw.ab, sw.ldab, row, col), b = load2<kF16>(sw.ab, sw.ldab, row, sw.Hp + col);
     const float s0 = sigmoid(a.x), s1 = sigmoid(a.y);
@@ -217,10 +228,42 @@ __device__ __forceinline__ void swiglu_bwd_pair(const SwigluArgs &sw, int row, i
     if (sw.h && in0) store2<kF16>(sw.h, sw.ldh, row, col, a.x * s0 * b.x, a.y * s1 * b.y, in1);
 }
 
+// GELU epilogues of one thread's fragment (see kEpiGeluFwd / kEpiGeluBwd).  Hp is a multiple of 8 and every pitch covers
+// it, so both columns of a pair are stored; pads hold p = 0, whose gelu and dpre are 0.  h is gelu of the rounded p in both,
+// so it equals F.gelu(pre) and the backward's recomputed h is the forward's, bit for bit.
+
+// gelu'(p) = Phi(p) + p phi(p).  Phi is taken from erfc, which does not cancel in the negative tail as 1 + erf does.  The
+// sum has a root at p = -0.7518: around it fp32 cancels to a relative error above half an fp16 ulp, so where
+// |factor| < 2^-8 (a few representable p) it is recomputed in fp64.
+__device__ __noinline__ float dgelu_f64(float p) {
+    const double q = (double)p;
+    return (float)(0.5 * erfc(-q * 0.70710678118654752) + q * exp(-0.5 * q * q) * 0.39894228040143268);
+}
+__device__ __forceinline__ float dgelu(float p) {
+    const float f = 0.5f * erfcf(-p * 0.70710678118654752f) + p * expf(-0.5f * p * p) * 0.3989422804014327f;
+    return fabsf(f) < 0.00390625f ? dgelu_f64(p) : f;
+}
+
+template <bool kF16>
+__device__ __forceinline__ void gelu_fwd_pair(const EpiArgs &ep, int row, int col, float acc0, float acc1, float b0, float b1) {
+    const bool in0 = col < ep.H, in1 = col + 1 < ep.H;
+    const float p0 = in0 ? round_to<kF16>(acc0 + b0) : 0.f, p1 = in1 ? round_to<kF16>(acc1 + b1) : 0.f;
+    if (ep.ab) store2<kF16>(ep.ab, ep.ldab, row, col, p0, p1, true);
+    store2<kF16>(ep.h, ep.ldh, row, col, gelu(p0), gelu(p1), true);
+}
+
+template <bool kF16>
+__device__ __forceinline__ void gelu_bwd_pair(const EpiArgs &ep, int row, int col, float g0, float g1) {
+    const bool in0 = col < ep.H, in1 = col + 1 < ep.H;
+    const float2 p = load2<kF16>(ep.ab, ep.ldab, row, col);
+    store2<kF16>(ep.dab, ep.lddab, row, col, in0 ? g0 * dgelu(p.x) : 0.f, in1 ? g1 * dgelu(p.y) : 0.f, true);
+    if (ep.h) store2<kF16>(ep.h, ep.ldh, row, col, in0 ? gelu(p.x) : 0.f, in1 ? gelu(p.y) : 0.f, true);
+}
+
 // The two consumer warpgroups: `cw` (0 / 1) owns rows [64 cw, 64 cw + 64) of every tile of this CTA.
 template <int BN, int kStages, bool kAMN, bool kBMN, bool kF16, int kEpi = kEpiLinear>
 __device__ __forceinline__ void gemm_consumer(const GemmArgs &g, char *tiles, uint64_t *full, uint64_t *empty, int cw,
-                                              const SwigluArgs *sw = nullptr) {
+                                              const EpiArgs *sw = nullptr) {
     constexpr int kABytes = kBM * kBK * 2, kStageBytes = kABytes + BN * kBK * 2;
     constexpr int kUnit = BN >= 128 ? 128 : 64;          // columns per wgmma instruction
     const int t = threadIdx.x & 127, lane = t & 31;
@@ -279,17 +322,27 @@ __device__ __forceinline__ void gemm_consumer(const GemmArgs &g, char *tiles, ui
                     }
                 }
             }
-        } else if constexpr (kEpi == kEpiSwigluBwd) {
+        } else if constexpr (kEpi != kEpiLinear) {
 #pragma unroll
             for (int u = 0; u < BN / kUnit; ++u) {
 #pragma unroll
                 for (int j = 0; j < kUnit / 8; ++j) {
                     const int col = nb * BN + u * kUnit + 8 * j + 2 * (lane & 3);
                     if (col < sw->Hp) {
+                        float b0 = 0.f, b1 = 0.f;
+                        if constexpr (kEpi == kEpiGeluFwd) {
+                            b0 = sw->b1 && col < sw->H ? __ldg(sw->b1 + col) : 0.f;
+                            b1 = sw->b1 && col + 1 < sw->H ? __ldg(sw->b1 + col + 1) : 0.f;
+                        }
 #pragma unroll
                         for (int h = 0; h < 2; ++h) {
                             const int row = row0 + 8 * h;
-                            if (row < g.M) swiglu_bwd_pair<kF16>(*sw, row, col, d[u][4 * j + 2 * h], d[u][4 * j + 2 * h + 1]);
+                            if (row < g.M) {
+                                const float v0 = d[u][4 * j + 2 * h], v1 = d[u][4 * j + 2 * h + 1];
+                                if constexpr (kEpi == kEpiSwigluBwd) swiglu_bwd_pair<kF16>(*sw, row, col, v0, v1);
+                                else if constexpr (kEpi == kEpiGeluFwd) gelu_fwd_pair<kF16>(*sw, row, col, v0, v1, b0, b1);
+                                else gelu_bwd_pair<kF16>(*sw, row, col, v0, v1);
+                            }
                         }
                     }
                 }
@@ -320,7 +373,7 @@ __device__ __forceinline__ void gemm_consumer(const GemmArgs &g, char *tiles, ui
 // [n0, n0 + 128) from tmB into its first half and W2's from tmB2 into its second, n0 = 128 nb (tmB2 is unused otherwise).
 template <int BN, int kStages, bool kAMN, bool kBMN, bool kF16, int kEpi>
 __device__ __forceinline__ void gemm_cta(const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmB2, const GemmArgs &g,
-                                         const SwigluArgs *sw) {
+                                         const EpiArgs *sw) {
     extern __shared__ char smem_raw[];
     // SWIZZLE_128B tiles must sit on 1024-byte boundaries
     char *tiles = reinterpret_cast<char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -385,8 +438,16 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tn_kernel(const __grid_c
 // MN-major, tmB2 unused).
 template <int kEpi, int BN, int kStages, bool kBMN, bool kF16>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_swiglu_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                                                                      const __grid_constant__ CUtensorMap tmB2, const GemmArgs g, const SwigluArgs sw) {
+                                                                      const __grid_constant__ CUtensorMap tmB2, const GemmArgs g, const EpiArgs sw) {
     gemm_cta<BN, kStages, false, kBMN, kF16, kEpi>(tmA, tmB, tmB2, g, &sw);
+}
+
+// GELU MLP's fc1 (kEpiGeluFwd: A = x, tmB = W1, K-major) and fc2 dgrad (kEpiGeluBwd: A = dy, tmB = W2 read MN-major); the
+// same parameters as gemm_swiglu_kernel so that one launcher serves both (tmB2 unused).
+template <int kEpi, int BN, int kStages, bool kBMN, bool kF16>
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_gelu_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                                                                    const __grid_constant__ CUtensorMap tmB2, const GemmArgs g, const EpiArgs ep) {
+    gemm_cta<BN, kStages, false, kBMN, kF16, kEpi>(tmA, tmB, tmB2, g, &ep);
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------
@@ -441,25 +502,36 @@ int launch_gemm(const CUtensorMap &tmA, const CUtensorMap &tmB, GemmArgs &g, int
     return mia::launched(mia::kErrGemm, "gemm launch");
 }
 
-// g.N is the hidden width H; a paired-B tile (forward) spans BN / 2 hidden columns, a backward tile BN.
+// The kernel of a fused-epilogue mode (taking only its address instantiates only it).
 template <int kEpi, int BN, int kStages, bool kBMN, bool kF16>
-int launch_swiglu(const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmB2, GemmArgs &g, const SwigluArgs &sw, int sms,
-                  cudaStream_t stream) {
+constexpr auto epi_kernel() {
+    if constexpr (kEpi == kEpiGeluFwd || kEpi == kEpiGeluBwd) return &gemm_gelu_kernel<kEpi, BN, kStages, kBMN, kF16>;
+    else return &gemm_swiglu_kernel<kEpi, BN, kStages, kBMN, kF16>;
+}
+
+// Launch of a fused-epilogue kernel.  g.N is the hidden width H; a paired-B tile (SwiGLU forward) spans BN / 2 hidden
+// columns, every other tile BN.
+template <int kEpi, int BN, int kStages, bool kBMN, bool kF16>
+int launch_epi(const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmB2, GemmArgs &g, const EpiArgs &ep, int sms,
+               cudaStream_t stream) {
     constexpr int smem = kStages * (kBM * kBK * 2 + BN * kBK * 2) + 2 * kStages * 8 + 1024;
     constexpr int span = kEpi == kEpiSwigluFwd ? BN / 2 : BN;
-    auto k = &gemm_swiglu_kernel<kEpi, BN, kStages, kBMN, kF16>;
+    constexpr bool gelu = kEpi == kEpiGeluFwd || kEpi == kEpiGeluBwd;
+    auto k = epi_kernel<kEpi, BN, kStages, kBMN, kF16>();
+    const char *name = gelu ? "gemm_gelu" : "gemm_swiglu";
     if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-        return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "cudaFuncSetAttribute(gemm_swiglu, %d B): %s", smem, cudaGetErrorString(cudaGetLastError()));
+        return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "cudaFuncSetAttribute(%s, %d B): %s", name, smem, cudaGetErrorString(cudaGetLastError()));
     g.num_m_blocks = (g.M + kBM - 1) / kBM;
     g.num_n_blocks = (g.N + span - 1) / span;
     g.num_k_blocks = (g.K + kBK - 1) / kBK;
     const int tiles = g.num_m_blocks * g.num_n_blocks;
     const int grid = tiles < sms ? tiles : sms;
-    k<<<grid, kGemmThreads, smem, stream>>>(tmA, tmB, tmB2, g, sw);
-    return mia::launched(mia::kErrGemm, "gemm_swiglu launch");
+    k<<<grid, kGemmThreads, smem, stream>>>(tmA, tmB, tmB2, g, ep);
+    return mia::launched(mia::kErrGemm, gelu ? "gemm_gelu launch" : "gemm_swiglu launch");
 }
 
 long long swiglu_pad(int H) { return ((long long)H + 63) / 64 * 64; }
+long long gelu_pad(int H) { return ((long long)H + 7) / 8 * 8; }
 
 }  // namespace
 
@@ -533,7 +605,7 @@ int mia_gemm_swiglu_fwd(const void *x, const void *w1, const void *w2, const flo
     GemmArgs g;
     memset(&g, 0, sizeof(g));
     g.M = M; g.N = H; g.K = K; g.in_f16 = dtype == MIA_GEMM_F16;
-    SwigluArgs sw;
+    EpiArgs sw;
     memset(&sw, 0, sizeof(sw));
     sw.b1 = b1; sw.b2 = b2; sw.h = h; sw.ab = ab; sw.ldh = ldh; sw.ldab = ldab; sw.H = H; sw.Hp = (int)Hp;
     CUtensorMap tmA, tmB, tmB2;
@@ -541,8 +613,8 @@ int mia_gemm_swiglu_fwd(const void *x, const void *w1, const void *w2, const flo
     if (int rc = make_map(&tmB, w1, H, K, ldw1, 128, dtype)) return rc;
     if (int rc = make_map(&tmB2, w2, H, K, ldw2, 128, dtype)) return rc;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
-    if (g.in_f16) return launch_swiglu<kEpiSwigluFwd, 256, 4, false, true>(tmA, tmB, tmB2, g, sw, di.sms, stream);
-    return launch_swiglu<kEpiSwigluFwd, 256, 4, false, false>(tmA, tmB, tmB2, g, sw, di.sms, stream);
+    if (g.in_f16) return launch_epi<kEpiSwigluFwd, 256, 4, false, true>(tmA, tmB, tmB2, g, sw, di.sms, stream);
+    return launch_epi<kEpiSwigluFwd, 256, 4, false, false>(tmA, tmB, tmB2, g, sw, di.sms, stream);
 }
 
 int mia_gemm_swiglu_bwd(const void *dy, const void *w3, const void *ab, void *dab, void *h, int M, int H, int N_out, long long lddy,
@@ -565,7 +637,7 @@ int mia_gemm_swiglu_bwd(const void *dy, const void *w3, const void *ab, void *da
     GemmArgs g;
     memset(&g, 0, sizeof(g));
     g.M = M; g.N = H; g.K = N_out; g.in_f16 = dtype == MIA_GEMM_F16;
-    SwigluArgs sw;
+    EpiArgs sw;
     memset(&sw, 0, sizeof(sw));
     sw.h = h; sw.ab = const_cast<void *>(ab); sw.dab = dab; sw.ldh = ldh; sw.ldab = ldab; sw.lddab = lddab; sw.H = H; sw.Hp = (int)Hp;
     // g = dy . W3: dy [M][N_out] K-major; W3 [N_out][H] read MN-major (rows = k), as LinearTC's dgrad reads it
@@ -575,11 +647,79 @@ int mia_gemm_swiglu_bwd(const void *dy, const void *w3, const void *ab, void *da
     const bool wide = (long long)((M + 127) / 128) * ((H + 255) / 256) >= di.sms;      // gemm_impl's choice between 128 and 256
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (g.in_f16) {
-        if (wide) return launch_swiglu<kEpiSwigluBwd, 256, 4, true, true>(tmA, tmB, tmB, g, sw, di.sms, stream);
-        return launch_swiglu<kEpiSwigluBwd, 128, 6, true, true>(tmA, tmB, tmB, g, sw, di.sms, stream);
+        if (wide) return launch_epi<kEpiSwigluBwd, 256, 4, true, true>(tmA, tmB, tmB, g, sw, di.sms, stream);
+        return launch_epi<kEpiSwigluBwd, 128, 6, true, true>(tmA, tmB, tmB, g, sw, di.sms, stream);
     }
-    if (wide) return launch_swiglu<kEpiSwigluBwd, 256, 4, true, false>(tmA, tmB, tmB, g, sw, di.sms, stream);
-    return launch_swiglu<kEpiSwigluBwd, 128, 6, true, false>(tmA, tmB, tmB, g, sw, di.sms, stream);
+    if (wide) return launch_epi<kEpiSwigluBwd, 256, 4, true, false>(tmA, tmB, tmB, g, sw, di.sms, stream);
+    return launch_epi<kEpiSwigluBwd, 128, 6, true, false>(tmA, tmB, tmB, g, sw, di.sms, stream);
+}
+
+int mia_gemm_gelu_fwd(const void *x, const void *w1, const float *b1, void *h, void *pre, int M, int H, int K, long long ldx, long long ldw1,
+                      long long ldh, long long ldpre, int dtype, void *cuda_stream) {
+    if (!x || !w1 || !h) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_fwd: null pointer (x, w1 and h are required)");
+    if (M <= 0 || H <= 0 || K <= 0) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_fwd: empty or negative size (M %d, H %d, K %d)", M, H, K);
+    if (dtype != MIA_GEMM_BF16 && dtype != MIA_GEMM_F16) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_fwd: dtype must be bf16 or fp16");
+    if ((ldx | ldw1 | ldh) % 8 || (pre && ldpre % 8) || ldx < K || ldw1 < K || ldh < H || (pre && ldpre < H))
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_fwd: row pitches must cover a row and be multiples of 8 elements "
+                         "(ldx %lld, ldw1 %lld, ldh %lld, ldpre %lld, H %d, K %d)", ldx, ldw1, ldh, ldpre, H, K);
+    if (((uintptr_t)x | (uintptr_t)w1 | (uintptr_t)h | (uintptr_t)pre) & 15)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_fwd: x, w1, h and pre must be 16-byte aligned");
+    mia::DeviceInfo di;
+    if (mia::device_info(mia::kErrGemm, di) != MIA_OK) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "gemm_gelu_fwd: cannot query the device");
+    GemmArgs g;
+    memset(&g, 0, sizeof(g));
+    g.M = M; g.N = H; g.K = K; g.in_f16 = dtype == MIA_GEMM_F16;
+    EpiArgs ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.b1 = b1; ep.h = h; ep.ab = pre; ep.ldh = ldh; ep.ldab = ldpre; ep.H = H; ep.Hp = (int)gelu_pad(H);
+    // gemm_impl's tile width for N = H, so pre has mia_gemm_tn's k order
+    const int BN = H <= 64 ? 64 : (H <= 128 || (long long)((M + 127) / 128) * ((H + 255) / 256) < di.sms ? 128 : 256);
+    CUtensorMap tmA, tmB;
+    if (int rc = make_map(&tmA, x, M, K, ldx, kBM, dtype)) return rc;
+    if (int rc = make_map(&tmB, w1, H, K, ldw1, BN, dtype)) return rc;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+#define MIA_GELU_FWD(F16)                                                                                       \
+    switch (BN) {                                                                                               \
+        case 64: return launch_epi<kEpiGeluFwd, 64, 8, false, F16>(tmA, tmB, tmB, g, ep, di.sms, stream);       \
+        case 128: return launch_epi<kEpiGeluFwd, 128, 6, false, F16>(tmA, tmB, tmB, g, ep, di.sms, stream);     \
+        default: return launch_epi<kEpiGeluFwd, 256, 4, false, F16>(tmA, tmB, tmB, g, ep, di.sms, stream);      \
+    }
+    if (g.in_f16) { MIA_GELU_FWD(true) }
+    MIA_GELU_FWD(false)
+#undef MIA_GELU_FWD
+}
+
+int mia_gemm_gelu_bwd(const void *dy, const void *w2, const void *pre, void *dpre, void *h, int M, int H, int N_out, long long lddy,
+                      long long ldw2, long long ldpre, long long lddpre, long long ldh, int dtype, void *cuda_stream) {
+    if (!dy || !w2 || !pre || !dpre) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_bwd: null pointer (dy, w2, pre and dpre are required)");
+    if (M <= 0 || H <= 0 || N_out <= 0)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_bwd: empty or negative size (M %d, H %d, N_out %d)", M, H, N_out);
+    if (dtype != MIA_GEMM_BF16 && dtype != MIA_GEMM_F16) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_bwd: dtype must be bf16 or fp16");
+    if ((lddy | ldw2 | ldpre | lddpre) % 8 || (h && ldh % 8) || lddy < N_out || ldw2 < H || ldpre < H || lddpre < H || (h && ldh < H))
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_bwd: row pitches must cover a row and be multiples of 8 elements "
+                         "(lddy %lld, ldw2 %lld, ldpre %lld, lddpre %lld, ldh %lld, H %d, N_out %d)", lddy, ldw2, ldpre, lddpre, ldh, H, N_out);
+    if (((uintptr_t)dy | (uintptr_t)w2 | (uintptr_t)pre | (uintptr_t)dpre | (uintptr_t)h) & 15)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "gemm_gelu_bwd: dy, w2, pre, dpre and h must be 16-byte aligned");
+    mia::DeviceInfo di;
+    if (mia::device_info(mia::kErrGemm, di) != MIA_OK) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "gemm_gelu_bwd: cannot query the device");
+    GemmArgs g;
+    memset(&g, 0, sizeof(g));
+    g.M = M; g.N = H; g.K = N_out; g.in_f16 = dtype == MIA_GEMM_F16;
+    EpiArgs ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.h = h; ep.ab = const_cast<void *>(pre); ep.dab = dpre; ep.ldh = ldh; ep.ldab = ldpre; ep.lddab = lddpre; ep.H = H; ep.Hp = (int)gelu_pad(H);
+    // g = dy . W2: dy [M][N_out] K-major; W2 [N_out][H] read MN-major (rows = k), as LinearTC's dgrad reads it
+    CUtensorMap tmA, tmB;
+    if (int rc = make_map(&tmA, dy, M, N_out, lddy, kBM, dtype)) return rc;
+    if (int rc = make_map(&tmB, w2, N_out, H, ldw2, kBK, dtype)) return rc;
+    const bool wide = (long long)((M + 127) / 128) * ((H + 255) / 256) >= di.sms;      // gemm_impl's choice between 128 and 256
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    if (g.in_f16) {
+        if (wide) return launch_epi<kEpiGeluBwd, 256, 4, true, true>(tmA, tmB, tmB, g, ep, di.sms, stream);
+        return launch_epi<kEpiGeluBwd, 128, 6, true, true>(tmA, tmB, tmB, g, ep, di.sms, stream);
+    }
+    if (wide) return launch_epi<kEpiGeluBwd, 256, 4, true, false>(tmA, tmB, tmB, g, ep, di.sms, stream);
+    return launch_epi<kEpiGeluBwd, 128, 6, true, false>(tmA, tmB, tmB, g, ep, di.sms, stream);
 }
 
 }  // extern "C"

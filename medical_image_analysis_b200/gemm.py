@@ -12,6 +12,7 @@ fp32 activations (no autocast) are NOT silently rounded to bf16: they take ``F.l
 from __future__ import annotations
 
 import torch
+import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib
@@ -130,6 +131,136 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None = No
     lead = x.shape[:-1]
     y = LinearTC.apply(x.reshape(-1, x.shape[-1]), weight, bias, act, out_dtype)
     return y.view(*lead, weight.shape[0])
+
+
+def _pad8(n):
+    return (n + 7) // 8 * 8
+
+
+class GeluMlpFn(torch.autograd.Function):
+    """fc2(gelu(fc1(x))) (VMamba's channel-last ``Mlp``, timm's ``Mlp`` in the MAE) as ONE op on the wgmma GEMM: fc1 writes
+    ``pre`` and ``h = gelu(pre)`` from its epilogue (mia_gemm_gelu_fwd) and fc2 reads ``h`` in place.  The backward's fc2
+    dgrad writes ``dpre = g gelu'(pre)`` and the recomputed ``h`` from its epilogue (mia_gemm_gelu_bwd); dW2 = dy^T h,
+    dx = dpre . W1 and dW1 = dpre^T x follow with no transposed copies.  DESIGN.md section 3.15.
+
+    ``pre``, ``h`` and the output are bit-identical to ``gemm.linear``'s fc1, ``F.gelu`` and fc2 in training mode.  Saved
+    (checkpoint_lvl 0): x in the activation dtype and ``pre`` (M, Hp); level 1 keeps x only and reruns the forward kernel.
+    Both give the same bits.  Hp = H rounded up to 8; with nothing to differentiate, nothing is saved and ``pre`` is not
+    written."""
+
+    @staticmethod
+    @torch.amp.custom_fwd(device_type="cuda")
+    def forward(ctx, x, w1, b1, w2, b2, checkpoint_lvl, train):
+        if checkpoint_lvl not in (0, 1):
+            raise ValueError(f"checkpoint_lvl must be 0 or 1, got {checkpoint_lvl!r}")
+        if not x.is_cuda:
+            raise RuntimeError("gelu_mlp_fn: this build has no CPU path (x must be a CUDA tensor)")
+        T = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled() else x.dtype
+        if T not in (torch.bfloat16, torch.float16):
+            raise RuntimeError(f"gelu_mlp_fn: activations must be bfloat16 or float16, directly or under autocast (got {T})")
+        H, K = w1.shape
+        N = w2.shape[0]
+        if tuple(w2.shape) != (N, H) or x.shape[-1] != K:
+            raise RuntimeError(f"gelu_mlp_fn: shapes do not chain: x {tuple(x.shape)}, w1 {tuple(w1.shape)}, w2 {tuple(w2.shape)}")
+        if K % 8 or N % 8:
+            raise RuntimeError(f"gelu_mlp_fn: in_features ({K}) and out_features ({N}) must be multiples of 8")
+        lead = x.shape[:-1]
+        x2 = x.to(T).reshape(-1, K)
+        if not _mn_ok(x2):
+            x2 = x2.contiguous()
+        M, Hp = x2.shape[0], _pad8(H)
+        if M == 0:
+            raise RuntimeError("gelu_mlp_fn: empty input")
+        ctx.sizes = (M, H, Hp, K, N, T, checkpoint_lvl)
+        pre = torch.empty((M, Hp), dtype=T, device=x.device) if train else None
+        h = torch.empty((M, Hp), dtype=T, device=x.device)
+        GeluMlpFn._fc1(x2, w1, b1, pre, h, ctx)
+        w2p = GeluMlpFn._w2(w2, ctx)
+        y = torch.empty((M, N), dtype=T, device=x.device)
+        b2f = None if b2 is None else b2.detach().float().contiguous()
+        _lib.call("mia_gemm_tn", "gelu_mlp_fn fc2", x.device, h.data_ptr(), w2p.data_ptr(), None if b2f is None else b2f.data_ptr(), y.data_ptr(),
+                  M, N, H, h.stride(0), w2p.stride(0), y.stride(0), _lib.dtype_code(T), _lib.dtype_code(T), ACT_NONE)
+        if train:
+            ctx.save_for_backward(x2, w1, b1, w2, b2, *([pre] if checkpoint_lvl == 0 else []))
+            ctx.bias_dtypes = tuple(None if b is None else b.dtype for b in (b1, b2))
+        return y.view(*lead, N)
+
+    @staticmethod
+    def _fc1(x2, w1, b1, pre, h, ctx):
+        """mia_gemm_gelu_fwd: h = gelu(pre) and, when pre is given, pre = x W1^T + b1."""
+        M, H, Hp, K, N, T, _ = ctx.sizes
+        w1c = w1.to(T).contiguous()
+        b1f = None if b1 is None else b1.detach().float().contiguous()
+        _lib.call("mia_gemm_gelu_fwd", "gelu_mlp_fn", x2.device, x2.data_ptr(), w1c.data_ptr(), None if b1f is None else b1f.data_ptr(),
+                  h.data_ptr(), None if pre is None else pre.data_ptr(), M, H, K, x2.stride(0), w1c.stride(0), h.stride(0),
+                  0 if pre is None else pre.stride(0), _lib.dtype_code(T))
+
+    @staticmethod
+    def _w2(w2, ctx):
+        """W2 in the activation dtype with a row pitch that is a multiple of 8 (zero-padded to Hp columns when H is not)."""
+        M, H, Hp, K, N, T, _ = ctx.sizes
+        if H % 8 == 0:
+            return w2.to(T).contiguous()
+        w2p = torch.zeros((N, Hp), dtype=T, device=w2.device)
+        w2p[:, :H] = w2
+        return w2p
+
+    @staticmethod
+    @torch.amp.custom_bwd(device_type="cuda")
+    def backward(ctx, dy):
+        M, H, Hp, K, N, T, lvl = ctx.sizes
+        x2, w1, b1, w2, b2, *keep = ctx.saved_tensors
+        dev = x2.device
+        need_x, need_w1, need_b1, need_w2, need_b2 = ctx.needs_input_grad[:5]
+        dy2 = dy.to(T).reshape(M, N)
+        if not _mn_ok(dy2):
+            dy2 = dy2.contiguous()
+        h = torch.empty((M, Hp), dtype=T, device=dev) if need_w2 or lvl == 1 else None
+        if lvl == 0:
+            pre = keep[0]
+        else:                                                      # rerun the forward kernel: pre and h, bit for bit
+            pre = torch.empty((M, Hp), dtype=T, device=dev)
+            GeluMlpFn._fc1(x2, w1, b1, pre, h, ctx)
+        w2p = GeluMlpFn._w2(w2, ctx)
+        dpre = torch.empty((M, Hp), dtype=T, device=dev)
+        h_bwd = h if lvl == 0 else None
+        _lib.call("mia_gemm_gelu_bwd", "gelu_mlp_fn backward", dev, dy2.data_ptr(), w2p.data_ptr(), pre.data_ptr(), dpre.data_ptr(),
+                  None if h_bwd is None else h_bwd.data_ptr(), M, H, N, dy2.stride(0), w2p.stride(0), pre.stride(0), dpre.stride(0),
+                  Hp if h_bwd is None else h_bwd.stride(0), _lib.dtype_code(T))
+        del pre
+        dx = dw1 = db1 = dw2 = db2 = None
+        if need_w2:                                                # dW2 = dy^T h
+            dw2 = gemm(dy2, h[:, :H], True, True, torch.float32).to(w2.dtype)
+        del h
+        if need_b2 and b2 is not None:
+            db2 = dy2.sum(0, dtype=torch.float32).to(ctx.bias_dtypes[1])
+        dpre = dpre[:, :H]
+        if need_x:                                                 # dx = dpre . W1 (W1 read MN-major)
+            dx = gemm(dpre, w1.to(T).contiguous(), False, True).view(*dy.shape[:-1], K)
+        if need_w1:                                                # dW1 = dpre^T x
+            dw1 = gemm(dpre, x2, True, True, torch.float32).to(w1.dtype)
+        if need_b1 and b1 is not None:
+            db1 = dpre.sum(0, dtype=torch.float32).to(ctx.bias_dtypes[0])
+        return dx, dw1, db1, dw2, db2, None, None
+
+
+def gelu_mlp_fn(x, w1, b1, w2, b2, checkpoint_lvl=0):
+    """fc2(gelu(fc1(x))) for bf16 / fp16 CUDA activations (directly or under autocast) as one op: x (..., in), w1 (H, in),
+    w2 (out, H) with in and out multiples of 8 (any H), biases (H) / (out) or None.  checkpoint_lvl 0 (default) keeps the
+    pre-activation for the backward, 1 recomputes it; both give the same bits."""
+    train = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, w1, b1, w2, b2))
+    return GeluMlpFn.apply(x, w1, b1, w2, b2, checkpoint_lvl, train)
+
+
+def gelu_mlp_eligible(mlp: nn.Module, x: torch.Tensor, dropout_off: bool) -> bool:
+    """Whether an fc1 -> GELU -> fc2 MLP (vmamba / mae ``Mlp``) runs as one op (gelu_mlp_fn): a backward follows (grad
+    enabled and an input or parameter requires it), bf16 / fp16 CUDA activations (directly or under autocast), nn.Linear
+    layers with in / out features multiples of 8, exact GELU and no active dropout inside."""
+    T = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled() and x.is_cuda else x.dtype
+    return (torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in mlp.parameters())) and x.is_cuda
+            and T in (torch.bfloat16, torch.float16) and type(mlp.fc1) is nn.Linear and type(mlp.fc2) is nn.Linear
+            and type(mlp.act) is nn.GELU and mlp.act.approximate == "none" and dropout_off and x.numel() > 0
+            and mlp.fc1.in_features % 8 == 0 and mlp.fc2.out_features % 8 == 0)
 
 
 def conv2d_patch(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor | None, stride, act: int = ACT_NONE) -> torch.Tensor:

@@ -63,7 +63,8 @@ class Attention(nn.Module):
 
 
 class Mlp(nn.Module):
-    """timm 0.9.2 ``layers.Mlp``: fc1 -> GELU -> fc2."""
+    """timm 0.9.2 ``layers.Mlp``: fc1 -> GELU -> fc2.  When a backward follows, bf16 / fp16 CUDA activations run it as one op
+    (gemm.gelu_mlp_fn); every other case runs the composition, _forward_composed."""
 
     def __init__(self, in_features, hidden_features):
         super().__init__()
@@ -72,6 +73,11 @@ class Mlp(nn.Module):
         self.fc2 = nn.Linear(hidden_features, in_features)
 
     def forward(self, x):
+        if _gemm.gelu_mlp_eligible(self, x, True):
+            return _gemm.gelu_mlp_fn(x, self.fc1.weight, self.fc1.bias, self.fc2.weight, self.fc2.bias)
+        return self._forward_composed(x)
+
+    def _forward_composed(self, x):
         return _gemm.linear(_gemm.linear(x, self.fc1.weight, self.fc1.bias, _gemm.ACT_GELU), self.fc2.weight, self.fc2.bias)
 
 

@@ -880,7 +880,9 @@ _ACT_CODE = {nn.ReLU: 1, nn.GELU: 2, nn.SiLU: 3}
 
 
 class Mlp(nn.Module):
-    """vmamba.py:495-514."""
+    """vmamba.py:495-514.  Channel-last with exact GELU, when a backward follows and no dropout is active, the layer runs as
+    one op (gemm.gelu_mlp_fn); every other case runs the composition, _forward_composed (no-grad inference included, which
+    already has the GELU in fc1's epilogue)."""
 
     def __init__(self, in_features, hidden_features=None, out_features=None, act_layer=nn.GELU, drop=0.0, channels_first=False):
         super().__init__()
@@ -892,6 +894,11 @@ class Mlp(nn.Module):
         self.drop = nn.Dropout(drop)
 
     def forward(self, x):
+        if _gemm.gelu_mlp_eligible(self, x, self.drop.p == 0 or not self.training):
+            return self.drop(_gemm.gelu_mlp_fn(x, self.fc1.weight, self.fc1.bias, self.fc2.weight, self.fc2.bias))
+        return self._forward_composed(x)
+
+    def _forward_composed(self, x):
         code = _ACT_CODE.get(type(self.act), None)
         if code in (1, 2) and type(self.fc1) is nn.Linear:      # activation fused into the GEMM epilogue
             x = _lin(self.fc1, x, code)
