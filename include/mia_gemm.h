@@ -73,6 +73,22 @@ int mia_gemm_gelu_fwd(const void *x, const void *w1, const float *b1, void *h, v
                       long long ldh, long long ldpre, int dtype, void *cuda_stream);
 int mia_gemm_gelu_bwd(const void *dy, const void *w2, const void *pre, void *dpre, void *h, int M, int H, int N_out, long long lddy,
                       long long ldw2, long long ldpre, long long lddpre, long long ldh, int dtype, void *cuda_stream);
+/* ViT-MAE attention (timm Attention: softmax(q k^T dh^-0.5) v per image and head, no mask, no dropout) on wgmma + TMA.
+ * C = H dh.  qkv is the qkv GEMM's output read in place: (B, N, 3, H, dh), row pitch ld_qkv >= 3C, q / k / v of head h in
+ * columns h dh, C + h dh, 2C + h dh.  Rows past token N - 1 of an image are never read as keys or written.
+ *
+ * Forward: o (B, N, C, pitch ld_o >= C) token-major, the layout the proj GEMM consumes; P is rounded to dtype before P V
+ * and O / l once.  lse (B, H, N) fp32 = logsumexp of the scaled logits per query row; NULL (inference) writes none.
+ *
+ * Backward: from dout = dL/do (B, N, C, pitch ld_do) writes dq / dk / dv straight into the packed dqkv (B, N, 3C, pitch
+ * ld_dqkv), the layout of qkv, i.e. the qkv GEMM's output gradient.  delta (B, H, N) fp32 is caller-owned scratch
+ * (rowsum(dout o o)).  Two launches (dq, then dk / dv), no atomics: the results are bit-reproducible.
+ *
+ * dh is 32, 64 or 80; B, N, H >= 1; dtype MIA_GEMM_BF16 or MIA_GEMM_F16 for every 16-bit operand; pitches multiples of 8
+ * elements covering a row; pointers 16-byte aligned.  Errors as for mia_gemm_tn. */
+int mia_attn_fwd(const void *qkv, void *o, float *lse, int B, int N, int H, int dh, long long ld_qkv, long long ld_o, int dtype, void *cuda_stream);
+int mia_attn_bwd(const void *qkv, const void *o, const void *dout, const float *lse, float *delta, void *dqkv, int B, int N, int H, int dh,
+                 long long ld_qkv, long long ld_o, long long ld_do, long long ld_dqkv, int dtype, void *cuda_stream);
 const char *mia_gemm_last_error(void);
 
 #ifdef __cplusplus

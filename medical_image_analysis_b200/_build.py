@@ -14,7 +14,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 SOURCES = ["scan_fwd_bf16.cu", "scan_fwd_f16.cu", "scan_fwd_f32.cu", "scan_bwd_bf16.cu", "scan_bwd_f16.cu", "scan_bwd_f32.cu",
            "scan_api.cu", "cross_scan.cu", "causal_conv1d.cu", "dwconv2d.cu", "gemm_wgmma.cu", "ssm_step.cu",
-           "ss2d_core.cu", "abi_host.cu"]
+           "ss2d_core.cu", "attention.cu", "abi_host.cu"]
 HEADERS = sorted(f for f in os.listdir(os.path.join(PKG, "csrc")) if f.endswith((".cuh", ".h"))) + [os.path.join("..", "..", "include", "mia_selective_scan.h"), os.path.join("..", "..", "include", "mia_gemm.h")]
 LIB = os.path.join(PKG, "libmia_scan.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

@@ -113,6 +113,8 @@ ABI = {
     "mia_gemm_swiglu_bwd": ([_vp] * 5 + [_I] * 3 + [_LL] * 5 + [_I, _vp], _I, _GEMM),
     "mia_gemm_gelu_fwd": ([_vp] * 5 + [_I] * 3 + [_LL] * 4 + [_I, _vp], _I, _GEMM),
     "mia_gemm_gelu_bwd": ([_vp] * 5 + [_I] * 3 + [_LL] * 5 + [_I, _vp], _I, _GEMM),
+    "mia_attn_fwd": ([_vp] * 3 + [_I] * 4 + [_LL] * 2 + [_I, _vp], _I, _GEMM),
+    "mia_attn_bwd": ([_vp] * 6 + [_I] * 4 + [_LL] * 4 + [_I, _vp], _I, _GEMM),
 }
 
 DTYPE_CODES = {torch.float32: MIA_F32, torch.float16: MIA_F16, torch.bfloat16: MIA_BF16}

@@ -41,6 +41,10 @@ int device_info(ErrChannel ch, DeviceInfo &di) {
     int dev = 0;
     MIA_QUERY(cudaGetDevice(&dev));
     if (dev != cached_dev) {
+        // Binds the device's primary context to this thread.  cudaGetDevice alone does not, and the driver calls that follow
+        // (cuTensorMapEncodeTiled) fail with CUDA_ERROR_INVALID_CONTEXT on a thread whose first CUDA work is one of ours,
+        // e.g. autograd's device thread when a backward starts with one of our ops.
+        MIA_QUERY(cudaSetDevice(dev));
         MIA_QUERY(cudaDeviceGetAttribute(&cached.sms, cudaDevAttrMultiProcessorCount, dev));
         MIA_QUERY(cudaDeviceGetAttribute(&cached.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
         cached_dev = dev;

@@ -8,8 +8,9 @@ names and shapes are the reference's (``patch_embed.conv1/conv2/proj``, ``blocks
 
 The patch encode is three kernel == stride convolutions, i.e. three GEMMs over non-overlapping patches with ReLU fused
 into the epilogue: per 1280 x 1280 image (6400 x 256).(256 x 1024), (400 x 16384).(16384 x 1024), (400 x 1024).(1024 x
-1024) = 17.6 GFLOP.  qkv / proj / fc1 (+GELU) / fc2 of the blocks are the same kernel; the 61- / 401-token attention itself
-is torch's scaled_dot_product_attention (tiny next to the GEMMs, SURVEY 8a).
+1024) = 17.6 GFLOP.  qkv / proj / fc1 (+GELU) / fc2 of the blocks are the same kernel.  The 61- / 401-token attention of
+bf16 / fp16 blocks is one op, ``AttentionFn``: the qkv GEMM, wgmma attention kernels that read q / k / v in place, and the
+proj GEMM, with a backward free of atomics (DESIGN.md section 3.16).  fp32 blocks run torch's scaled_dot_product_attention.
 """
 from __future__ import annotations
 
@@ -21,6 +22,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from . import _lib
 from . import gemm as _gemm
 
 
@@ -44,7 +46,8 @@ class SmallPatchEmbed(nn.Module):
 
 
 class Attention(nn.Module):
-    """timm 0.9.2 ``vision_transformer.Attention`` (qkv_bias, no qk_norm, no dropout)."""
+    """timm 0.9.2 ``vision_transformer.Attention`` (qkv_bias, no qk_norm, no dropout).  Runs as one op (attention_fn) where
+    attention_eligible says so; every other case runs the composition, _forward_composed."""
 
     def __init__(self, dim, num_heads=8, qkv_bias=False):
         super().__init__()
@@ -55,11 +58,115 @@ class Attention(nn.Module):
         self.proj = nn.Linear(dim, dim)
 
     def forward(self, x):
+        if attention_eligible(self, x):
+            return attention_fn(x, self.qkv.weight, self.qkv.bias, self.proj.weight, self.proj.bias, self.num_heads)
+        return self._forward_composed(x)
+
+    def _forward_composed(self, x):
         B, N, C = x.shape
         qkv = _gemm.linear(x, self.qkv.weight, self.qkv.bias).reshape(B, N, 3, self.num_heads, self.head_dim).permute(2, 0, 3, 1, 4)
         q, k, v = qkv.unbind(0)
         x = F.scaled_dot_product_attention(q, k, v)             # softmax(q k^T / sqrt(d)) v
         return _gemm.linear(x.transpose(1, 2).reshape(B, N, C), self.proj.weight, self.proj.bias)
+
+
+ATTN_HEAD_DIMS = (32, 64, 80)
+
+
+class AttentionFn(torch.autograd.Function):
+    """timm's Attention (proj(softmax(q k^T dh^-0.5) v) with qkv = x W_qkv^T + b_qkv) as ONE op: the qkv GEMM writes
+    (B, N, 3, H, dh), mia_attn_fwd reads q / k / v from it in place and writes o token-major (B, N, C), the layout the
+    proj GEMM reads.  The backward runs proj's dgrad / wgrad, mia_attn_bwd (two launches, no atomics) writing dq / dk / dv
+    into the packed (B, N, 3C) gradient of qkv, then qkv's dgrad / wgrad with no transposed copies; bias gradients are
+    fp32 column sums.  DESIGN.md section 3.16.
+
+    Saved (checkpoint_lvl 0): x in the activation dtype, qkv, o and the fp32 logsumexp (B, H, N); level 1 keeps x only and
+    reruns the qkv GEMM and the forward kernel.  Both give the same bits.  With nothing to differentiate, nothing is saved
+    and no logsumexp is written."""
+
+    @staticmethod
+    @torch.amp.custom_fwd(device_type="cuda")
+    def forward(ctx, x, qkv_weight, qkv_bias, proj_weight, proj_bias, num_heads, checkpoint_lvl, train):
+        if checkpoint_lvl not in (0, 1):
+            raise ValueError(f"checkpoint_lvl must be 0 or 1, got {checkpoint_lvl!r}")
+        if not x.is_cuda:
+            raise RuntimeError("attention_fn: this build has no CPU path (x must be a CUDA tensor)")
+        T = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled() else x.dtype
+        if T not in (torch.bfloat16, torch.float16):
+            raise RuntimeError(f"attention_fn: activations must be bfloat16 or float16, directly or under autocast (got {T})")
+        if x.dim() != 3 or x.numel() == 0:
+            raise RuntimeError(f"attention_fn: x must be a non-empty (B, N, C) tensor, got {tuple(x.shape)}")
+        B, N, C = x.shape
+        if C % num_heads or C // num_heads not in ATTN_HEAD_DIMS:
+            raise RuntimeError(f"attention_fn: head dim C / num_heads = {C} / {num_heads} must be one of {ATTN_HEAD_DIMS}")
+        if tuple(qkv_weight.shape) != (3 * C, C) or tuple(proj_weight.shape) != (C, C):
+            raise RuntimeError(f"attention_fn: weights {tuple(qkv_weight.shape)} / {tuple(proj_weight.shape)} do not match C = {C}")
+        x2 = x.to(T).reshape(B * N, C)
+        if not _gemm._mn_ok(x2):
+            x2 = x2.contiguous()
+        ctx.sizes = (B, N, C, num_heads, T, checkpoint_lvl)
+        qkv, o, lse = AttentionFn._attend(x2, qkv_weight, qkv_bias, ctx, train)
+        y = _gemm.gemm_tn(o, proj_weight.to(T), proj_bias)
+        if train:
+            ctx.save_for_backward(x2, qkv_weight, qkv_bias, proj_weight, proj_bias, *([qkv, o, lse] if checkpoint_lvl == 0 else []))
+            ctx.param_dtypes = tuple(None if t is None else t.dtype for t in (qkv_weight, qkv_bias, proj_weight, proj_bias))
+        return y.view(B, N, C)
+
+    @staticmethod
+    def _attend(x2, qkv_weight, qkv_bias, ctx, train):
+        """qkv = x W^T + b (bit-identical to gemm.linear), o and, when training, the logsumexp."""
+        B, N, C, H, T, _ = ctx.sizes
+        qkv = _gemm.gemm_tn(x2, qkv_weight.to(T), qkv_bias)
+        o = torch.empty((B * N, C), dtype=T, device=x2.device)
+        lse = torch.empty((B, H, N), dtype=torch.float32, device=x2.device) if train else None
+        _lib.call("mia_attn_fwd", "attention_fn", x2.device, qkv.data_ptr(), o.data_ptr(), None if lse is None else lse.data_ptr(), B, N, H,
+                  C // H, qkv.stride(0), o.stride(0), _lib.dtype_code(T))
+        return qkv, o, lse
+
+    @staticmethod
+    @torch.amp.custom_bwd(device_type="cuda")
+    def backward(ctx, dy):
+        B, N, C, H, T, lvl = ctx.sizes
+        x2, wq, bq, wp, bp, *keep = ctx.saved_tensors
+        dev = x2.device
+        need_x, need_wq, need_bq, need_wp, need_bp = ctx.needs_input_grad[:5]
+        qkv, o, lse = keep if lvl == 0 else AttentionFn._attend(x2, wq, bq, ctx, True)
+        dy2 = dy.to(T).reshape(B * N, C)
+        if not _gemm._mn_ok(dy2):
+            dy2 = dy2.contiguous()
+        dx = dwq = dbq = dwp = dbp = None
+        if need_wp:                                                # dWp = dy^T o
+            dwp = _gemm.gemm(dy2, o, True, True, torch.float32).to(ctx.param_dtypes[2])
+        if need_bp and bp is not None:
+            dbp = dy2.sum(0, dtype=torch.float32).to(ctx.param_dtypes[3])
+        do = _gemm.gemm(dy2, wp.to(T).contiguous(), False, True)   # dO = dy . Wp (Wp read MN-major)
+        delta = torch.empty((B, H, N), dtype=torch.float32, device=dev)
+        dqkv = torch.empty((B * N, 3 * C), dtype=T, device=dev)
+        _lib.call("mia_attn_bwd", "attention_fn backward", dev, qkv.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr(), delta.data_ptr(),
+                  dqkv.data_ptr(), B, N, H, C // H, qkv.stride(0), o.stride(0), do.stride(0), dqkv.stride(0), _lib.dtype_code(T))
+        del qkv, o, lse, do, delta
+        if need_x:                                                 # dx = dqkv . Wq (Wq read MN-major)
+            dx = _gemm.gemm(dqkv, wq.to(T).contiguous(), False, True).view(B, N, C)
+        if need_wq:                                                # dWq = dqkv^T x
+            dwq = _gemm.gemm(dqkv, x2, True, True, torch.float32).to(ctx.param_dtypes[0])
+        if need_bq and bq is not None:
+            dbq = dqkv.sum(0, dtype=torch.float32).to(ctx.param_dtypes[1])
+        return dx, dwq, dbq, dwp, dbp, None, None, None
+
+
+def attention_fn(x, qkv_weight, qkv_bias, proj_weight, proj_bias, num_heads, checkpoint_lvl=0):
+    """timm's Attention for bf16 / fp16 CUDA activations (directly or under autocast) as one op: x (B, N, C), qkv_weight
+    (3C, C), proj_weight (C, C), biases (3C) / (C) or None, head dim C / num_heads in ATTN_HEAD_DIMS.  checkpoint_lvl 0
+    (default) keeps qkv, o and the logsumexp for the backward, 1 recomputes them; both give the same bits."""
+    train = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, qkv_weight, qkv_bias, proj_weight, proj_bias))
+    return AttentionFn.apply(x, qkv_weight, qkv_bias, proj_weight, proj_bias, num_heads, checkpoint_lvl, train)
+
+
+def attention_eligible(attn: nn.Module, x: torch.Tensor) -> bool:
+    """Whether an Attention runs as one op (attention_fn): CUDA tensors, bf16 / fp16 activations (directly or under autocast)
+    and a head dim in ATTN_HEAD_DIMS, with or without grad."""
+    T = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled() and x.is_cuda else x.dtype
+    return x.is_cuda and T in (torch.bfloat16, torch.float16) and attn.head_dim in ATTN_HEAD_DIMS and x.dim() == 3 and x.numel() > 0
 
 
 class Mlp(nn.Module):
