@@ -590,7 +590,7 @@ int mia_gemm_swiglu_bwd(const void *dy, const void *w3, const void *ab, void *da
     CUtensorMap tmA, tmB;
     if (int rc = make_map(&tmA, dy, M, N_out, lddy, kBM, dtype)) return rc;
     if (int rc = make_map(&tmB, w3, N_out, H, ldw3, kBK, dtype)) return rc;
-    const bool wide = (long long)((M + 127) / 128) * ((H + 255) / 256) >= di.sms;      // gemm_impl's choice between 128 and 256
+    const bool wide = H > 128 && (long long)((M + 127) / 128) * ((H + 255) / 256) >= di.sms;      // gemm_impl's choice between 128 and 256
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (g.in_f16) {
         if (wide) return launch_epi<kEpiSwigluBwd, 256, 4, true, true>(tmA, tmB, tmB, g, sw, di.sms, stream);
@@ -658,7 +658,7 @@ int mia_gemm_gelu_bwd(const void *dy, const void *w2, const void *pre, void *dpr
     CUtensorMap tmA, tmB;
     if (int rc = make_map(&tmA, dy, M, N_out, lddy, kBM, dtype)) return rc;
     if (int rc = make_map(&tmB, w2, N_out, H, ldw2, kBK, dtype)) return rc;
-    const bool wide = (long long)((M + 127) / 128) * ((H + 255) / 256) >= di.sms;      // gemm_impl's choice between 128 and 256
+    const bool wide = H > 128 && (long long)((M + 127) / 128) * ((H + 255) / 256) >= di.sms;      // gemm_impl's choice between 128 and 256
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     if (g.in_f16) {
         if (wide) return launch_epi<kEpiGeluBwd, 256, 4, true, true>(tmA, tmB, tmB, g, ep, di.sms, stream);
