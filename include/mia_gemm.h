@@ -89,6 +89,22 @@ int mia_gemm_gelu_bwd(const void *dy, const void *w2, const void *pre, void *dpr
 int mia_attn_fwd(const void *qkv, void *o, float *lse, int B, int N, int H, int dh, long long ld_qkv, long long ld_o, int dtype, void *cuda_stream);
 int mia_attn_bwd(const void *qkv, const void *o, const void *dout, const float *lse, float *delta, void *dqkv, int B, int N, int H, int dh,
                  long long ld_qkv, long long ld_o, long long ld_do, long long ld_dqkv, int dtype, void *cuda_stream);
+/* Segment-causal cross-attention (the ARM pre-training decoder's CrossAttention: softmax(q k^T dh^-0.5 + mask) v with
+ * mask 0 where key // seg <= query // seg and -inf elsewhere) on the kernels above.  C = H dh, dh = 64.  q is the q GEMM's
+ * output (B, N, C, pitch ld_q >= C), kv the kv GEMM's output (B, N, 2C, pitch ld_kv >= 2C) with k / v of head h in columns
+ * h dh / C + h dh; both are read in place.  Key tiles that no query of a tile can see are skipped.
+ *
+ * Forward: o and lse as for mia_attn_fwd (lse NULL: inference).  Backward: dq into (B, N, C, pitch ld_dq >= C) and dk / dv
+ * into the packed (B, N, 2C, pitch ld_dkv >= 2C): the output gradients of the q and kv GEMMs.  delta (B, H, N) fp32 is
+ * caller-owned scratch.  No atomics: the results are bit-reproducible.
+ *
+ * 1 <= B, H <= 65535; N >= 1; 1 <= seg <= N; dtype MIA_GEMM_BF16 or MIA_GEMM_F16; pitches multiples of 8 elements covering
+ * a row; pointers 16-byte aligned.  Errors as for mia_gemm_tn. */
+int mia_xattn_fwd(const void *q, const void *kv, void *o, float *lse, int B, int N, int H, int dh, int seg, long long ld_q, long long ld_kv,
+                  long long ld_o, int dtype, void *cuda_stream);
+int mia_xattn_bwd(const void *q, const void *kv, const void *o, const void *dout, const float *lse, float *delta, void *dq, void *dkv, int B, int N,
+                  int H, int dh, int seg, long long ld_q, long long ld_kv, long long ld_o, long long ld_do, long long ld_dq, long long ld_dkv, int dtype,
+                  void *cuda_stream);
 const char *mia_gemm_last_error(void);
 
 #ifdef __cplusplus

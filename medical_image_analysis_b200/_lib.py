@@ -115,6 +115,8 @@ ABI = {
     "mia_gemm_gelu_bwd": ([_vp] * 5 + [_I] * 3 + [_LL] * 5 + [_I, _vp], _I, _GEMM),
     "mia_attn_fwd": ([_vp] * 3 + [_I] * 4 + [_LL] * 2 + [_I, _vp], _I, _GEMM),
     "mia_attn_bwd": ([_vp] * 6 + [_I] * 4 + [_LL] * 4 + [_I, _vp], _I, _GEMM),
+    "mia_xattn_fwd": ([_vp] * 4 + [_I] * 5 + [_LL] * 3 + [_I, _vp], _I, _GEMM),
+    "mia_xattn_bwd": ([_vp] * 8 + [_I] * 5 + [_LL] * 6 + [_I, _vp], _I, _GEMM),
 }
 
 DTYPE_CODES = {torch.float32: MIA_F32, torch.float16: MIA_F16, torch.bfloat16: MIA_BF16}

@@ -19,6 +19,16 @@
 //                       above, dV += P^T dO, dK += dS^T Q.  dk = round(dh^-0.5 dK), dv = round(dV).
 // Key columns >= N are -inf (forward) / P = 0 (backward) before anything else sees them; rows >= N are never stored.  No
 // atomics: every output element is summed in a fixed order, so results are bit-reproducible.
+//
+// Cross-attention (kX = true; the ARM pre-training decoder's CrossAttention, CXPMRG_Bench_MambaXray_VL/pretrain/
+// models_pretrain.py:55-83, 395-400): q is the q GEMM's output (B, N, C) read through its own map (C, N, B), k / v the kv
+// GEMM's output (B, N, 2C) through one map (2C, N, B) at columns h dh / C + h dh.  A segment-causal mask of segment length
+// seg: key j is visible to query i iff j / seg <= i / seg, i.e. j < (i / seg + 1) seg.  Masked scores become -inf before
+// the row max (a select, not an add) and P = 0 in the backward.  Key 0 is visible to every row, so the running max is
+// finite after the first key tile and a later tile that a row cannot see adds exact zeros.  Tiles no row of a CTA can see
+// are skipped: the forward / dq loops end at the key tile holding the last key visible to the CTA's last valid query row,
+// and the dkv loop starts at the query tile holding the first query that sees the CTA's first key.  dq goes to (B, N, C)
+// and dk / dv to a packed (B, N, 2C): the output gradients of the q and kv GEMMs.  Head dim 64 only.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -43,9 +53,35 @@ struct AttnArgs {
     const void *dout;
     const float *lse;                     // backward input
     float *lse_out, *delta;               // forward output (may be NULL) / backward scratch
-    void *dqkv;
+    void *dqkv;                           // self-attention: the packed dqkv; cross-attention: dq (B, N, C)
     long long ld_o, ld_do, ld_dqkv;
+    void *dkv;                            // cross-attention: the packed (B, N, 2C) dk / dv
+    long long ld_dkv;
+    int seg;                              // cross-attention: segment length of the mask
 };
+
+// The tensor maps of a launch: self-attention reads q / k / v from one map (3C, N, B) at columns h dh, C + h dh, 2C + h dh;
+// cross-attention reads q from m[0] (C, N, B) at h dh and k / v from m[1] (2C, N, B) at h dh, C + h dh.
+template <bool kX>
+struct Maps {
+    CUtensorMap m[kX ? 2 : 1];
+};
+template <bool kX>
+__device__ __forceinline__ const CUtensorMap *map_kv(const Maps<kX> &tm) { return &tm.m[kX ? 1 : 0]; }
+template <bool kX, int DH>
+__device__ __forceinline__ int col_k(const AttnArgs &a, int head) { return (kX ? 0 : a.C) + head * DH; }
+template <bool kX, int DH>
+__device__ __forceinline__ int col_v(const AttnArgs &a, int head) { return (kX ? a.C : 2 * a.C) + head * DH; }
+
+// One past the last key visible to query i under the segment-causal mask, capped at N.
+__device__ __forceinline__ int seg_end(int i, int seg, int N) { return min(N, (i / seg + 1) * seg); }
+
+// Key tiles a CTA of query tile qt visits: all of them, or (kX) up to the one holding the last key its last valid row sees.
+template <bool kX>
+__device__ __forceinline__ int key_steps(const AttnArgs &a, int qt) {
+    if (!kX) return (a.N + kRows - 1) / kRows;
+    return (seg_end(min(a.N, (qt + 1) * kRows) - 1, a.seg, a.N) + kRows - 1) / kRows;
+}
 
 // d[64 x N fragment] += A[registers, 64 x 16] . B[smem desc, 16 x N], B MN-major (its N index contiguous).  A fragment of
 // thread t: a[0] = (row g, k 2q..2q+1), a[1] = (g + 8, same k), a[2] = (g, 2q + 8..), a[3] = (g + 8, 2q + 8..), with
@@ -154,10 +190,10 @@ __device__ __forceinline__ Ring setup_ring(int fixed) {
 }
 
 // The producer (lane 0 of warp 4): the two fixed tiles (columns fcol0 / fcol1 of maps fm0 / fm1, rows frow), then for
-// each of `steps` row tiles the pair (columns scol0 of sm0, scol1 of sm1).
+// each of the row tiles [first, steps) the pair (columns scol0 of sm0, scol1 of sm1).
 template <int DH>
 __device__ __forceinline__ void produce(const Ring &r, const CUtensorMap *fm0, int fcol0, const CUtensorMap *fm1, int fcol1, int frow, int nfixed,
-                                        const CUtensorMap *sm0, int scol0, const CUtensorMap *sm1, int scol1, int steps, int b) {
+                                        const CUtensorMap *sm0, int scol0, const CUtensorMap *sm1, int scol1, int first, int steps, int b) {
     constexpr int kTile = kRows * DH * 2;
     asm volatile("prefetch.tensormap [%0];" ::"l"(fm0) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(sm1) : "memory");
@@ -166,7 +202,7 @@ __device__ __forceinline__ void produce(const Ring &r, const CUtensorMap *fm0, i
     if (nfixed == 2) load_tile<DH>(r.fixed + kTile, fm1, fcol1, frow, b, r.fbar);
     int s = 0;
     uint32_t ph = 0;
-    for (int i = 0; i < steps; ++i) {
+    for (int i = first; i < steps; ++i) {
         mia::mbar_wait(r.empty + s, ph ^ 1);
         mia::mbar_arrive_expect_tx(r.full + s, 2 * kTile);
         char *st = r.stages + s * 2 * kTile;
@@ -176,18 +212,25 @@ __device__ __forceinline__ void produce(const Ring &r, const CUtensorMap *fm0, i
     }
 }
 
-template <int DH, bool kF16>
-__global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const AttnArgs a) {
+template <int DH, bool kF16, bool kX>
+__global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constant__ Maps<kX> tm, const AttnArgs a) {
     constexpr int kTile = kRows * DH * 2;
     const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z, N = a.N;
-    const int steps = (N + kRows - 1) / kRows;
+    const int steps = key_steps<kX>(a, qt);
     const Ring r = setup_ring<DH>(1);
     if (threadIdx.x >= 128) {
         if (threadIdx.x == 128)
-            produce<DH>(r, &tm_qkv, head * DH, &tm_qkv, 0, qt * kRows, 1, &tm_qkv, a.C + head * DH, &tm_qkv, 2 * a.C + head * DH, steps, b);
+            produce<DH>(r, &tm.m[0], head * DH, &tm.m[0], 0, qt * kRows, 1, map_kv(tm), col_k<kX, DH>(a, head), map_kv(tm), col_v<kX, DH>(a, head), 0, steps, b);
         return;
     }
     const int t = threadIdx.x, q = t & 3;
+    int lim[2], lim0 = 0;                     // kX: one past the last visible key of rows rl, rl + 8, and of the CTA's first row
+    if constexpr (kX) {
+        const int row = qt * kRows + 16 * (t >> 5) + ((t & 31) >> 2);
+        lim[0] = seg_end(row, a.seg, N);
+        lim[1] = seg_end(row + 8, a.seg, N);
+        lim0 = seg_end(qt * kRows, a.seg, N);
+    }
     float o[DH / 2], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 #pragma unroll
     for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
@@ -204,7 +247,17 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
         for (int kk = 0; kk < DH / 16; ++kk) mia::wgmma_n64<kF16, false, false>(sc, desc_k(aq, kk), desc_k(ak, kk), kk);
         mia::wgmma_commit();
         mia::wgmma_wait<0>();
-        if ((kt + 1) * kRows > N) {               // keys past N: zero-filled rows that would still score 0
+        if constexpr (kX) {
+            if ((kt + 1) * kRows > lim0) {        // keys a row cannot see (including those past N)
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int c = 0; c < 2; ++c)
+                            if (kt * kRows + 8 * j + 2 * q + c >= lim[h]) sc[4 * j + 2 * h + c] = -INFINITY;
+            }
+        } else if ((kt + 1) * kRows > N) {        // keys past N: zero-filled rows that would still score 0
 #pragma unroll
             for (int j = 0; j < 8; ++j)
 #pragma unroll
@@ -286,23 +339,26 @@ __device__ __forceinline__ void row_stats(const AttnArgs &a, int b, int head, in
     }
 }
 
-template <int DH, bool kF16>
-__global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
+template <int DH, bool kF16, bool kX>
+__global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_constant__ Maps<kX> tm, const __grid_constant__ CUtensorMap tm_do,
                                                              const AttnArgs a) {
     constexpr int kTile = kRows * DH * 2;
     __shared__ float lse_s[kRows], delta_s[kRows];
     const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z, N = a.N;
-    const int steps = (N + kRows - 1) / kRows;
+    const int steps = key_steps<kX>(a, qt);
     const Ring r = setup_ring<DH>(2);
     if (threadIdx.x >= 128) {
         if (threadIdx.x == 128)
-            produce<DH>(r, &tm_qkv, head * DH, &tm_do, head * DH, qt * kRows, 2, &tm_qkv, a.C + head * DH, &tm_qkv, 2 * a.C + head * DH, steps, b);
+            produce<DH>(r, &tm.m[0], head * DH, &tm_do, head * DH, qt * kRows, 2, map_kv(tm), col_k<kX, DH>(a, head), map_kv(tm), col_v<kX, DH>(a, head), 0,
+                        steps, b);
         return;
     }
     const int t = threadIdx.x, q = t & 3, rl = 16 * (t >> 5) + ((t & 31) >> 2);
     row_stats<DH, kF16>(a, b, head, qt * kRows, lse_s, delta_s);
     consumer_sync();
     const float lse2[2] = {lse_s[rl], lse_s[rl + 8]}, dlt[2] = {delta_s[rl], delta_s[rl + 8]};
+    // one past the last visible key of rows rl, rl + 8
+    const int lim[2] = {kX ? seg_end(qt * kRows + rl, a.seg, N) : N, kX ? seg_end(qt * kRows + rl + 8, a.seg, N) : N};
     float dq[DH / 2];
 #pragma unroll
     for (int i = 0; i < DH / 2; ++i) dq[i] = 0.f;
@@ -328,7 +384,7 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
 #pragma unroll
                 for (int c = 0; c < 2; ++c) {
                     const int i = 4 * j + 2 * h + c;
-                    const float p = kt * kRows + 8 * j + 2 * q + c < N ? exp2f(fmaf(sc[i], a.scale_log2, -lse2[h])) : 0.f;
+                    const float p = kt * kRows + 8 * j + 2 * q + c < lim[h] ? exp2f(fmaf(sc[i], a.scale_log2, -lse2[h])) : 0.f;
                     sc[i] = p * (dp[i] - dlt[h]);
                 }
         uint32_t da[4][4];
@@ -344,19 +400,27 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
     store_rows<DH, kF16>(a.dqkv, a.ld_dqkv, b, N, qt * kRows, head * DH, dq, a.scale);
 }
 
-template <int DH, bool kF16>
-__global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
+template <int DH, bool kF16, bool kX>
+__global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_constant__ Maps<kX> tm, const __grid_constant__ CUtensorMap tm_do,
                                                               const AttnArgs a) {
     constexpr int kTile = kRows * DH * 2;
     const int kt = blockIdx.x, head = blockIdx.y, b = blockIdx.z, N = a.N;
     const int steps = (N + kRows - 1) / kRows;
+    const int first = kX ? kt * kRows / a.seg * a.seg / kRows : 0;     // kX: the query tile of the first query that sees key kt 64
     const Ring r = setup_ring<DH>(2);
     if (threadIdx.x >= 128) {
         if (threadIdx.x == 128)
-            produce<DH>(r, &tm_qkv, a.C + head * DH, &tm_qkv, 2 * a.C + head * DH, kt * kRows, 2, &tm_qkv, head * DH, &tm_do, head * DH, steps, b);
+            produce<DH>(r, map_kv(tm), col_k<kX, DH>(a, head), map_kv(tm), col_v<kX, DH>(a, head), kt * kRows, 2, &tm.m[0], head * DH, &tm_do, head * DH,
+                        first, steps, b);
         return;
     }
     const int t = threadIdx.x, q = t & 3;
+    int lo[2] = {0, 0};                       // kX: the first query that sees key rows rl, rl + 8
+    if constexpr (kX) {
+        const int key = kt * kRows + 16 * (t >> 5) + ((t & 31) >> 2);
+        lo[0] = key / a.seg * a.seg;
+        lo[1] = (key + 8) / a.seg * a.seg;
+    }
     const float *lse = a.lse + ((size_t)b * a.H + head) * N, *delta = a.delta + ((size_t)b * a.H + head) * N;
     float dk[DH / 2], dv[DH / 2];
 #pragma unroll
@@ -365,7 +429,7 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
     mia::mbar_wait(r.fbar, 0);
     int s = 0;
     uint32_t ph = 0;
-    for (int it = 0; it < steps; ++it) {
+    for (int it = first; it < steps; ++it) {
         mia::mbar_wait(r.full + s, ph);
         const uint32_t aq = mia::smem_u32(r.stages + s * 2 * kTile), ado = aq + kTile;
         float sc[32], dp[32];
@@ -386,7 +450,7 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const int i = 4 * j + 2 * h + c;
-                    const float p = in ? exp2f(fmaf(sc[i], a.scale_log2, -lse2)) : 0.f;
+                    const float p = in && (!kX || col >= lo[h]) ? exp2f(fmaf(sc[i], a.scale_log2, -lse2)) : 0.f;
                     sc[i] = p;
                     dp[i] = p * (dp[i] - dlt);
                 }
@@ -404,8 +468,13 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
         if (t == 0) mia::mbar_arrive(r.empty + s);
         if (++s == kStages) { s = 0; ph ^= 1; }
     }
-    store_rows<DH, kF16>(a.dqkv, a.ld_dqkv, b, N, kt * kRows, a.C + head * DH, dk, a.scale);
-    store_rows<DH, kF16>(a.dqkv, a.ld_dqkv, b, N, kt * kRows, 2 * a.C + head * DH, dv, 1.f);
+    if constexpr (kX) {
+        store_rows<DH, kF16>(a.dkv, a.ld_dkv, b, N, kt * kRows, head * DH, dk, a.scale);
+        store_rows<DH, kF16>(a.dkv, a.ld_dkv, b, N, kt * kRows, a.C + head * DH, dv, 1.f);
+    } else {
+        store_rows<DH, kF16>(a.dqkv, a.ld_dqkv, b, N, kt * kRows, a.C + head * DH, dk, a.scale);
+        store_rows<DH, kF16>(a.dqkv, a.ld_dqkv, b, N, kt * kRows, 2 * a.C + head * DH, dv, 1.f);
+    }
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------
@@ -445,17 +514,26 @@ int launch(K kernel, int smem, dim3 grid, cudaStream_t stream, const char *what,
     return mia::launched(mia::kErrGemm, what);
 }
 
-template <int DH, bool kF16>
-int launch_fwd(const CUtensorMap &tm, const AttnArgs &a, int B, cudaStream_t stream) {
+template <int DH, bool kF16, bool kX = false>
+int launch_fwd(const Maps<kX> &tm, const AttnArgs &a, int B, cudaStream_t stream) {
     const dim3 grid((a.N + kRows - 1) / kRows, a.H, B);
-    return launch(&attn_fwd_kernel<DH, kF16>, smem_bytes<DH>(1), grid, stream, "attn_fwd launch", tm, a);
+    return launch(&attn_fwd_kernel<DH, kF16, kX>, smem_bytes<DH>(1), grid, stream, kX ? "xattn_fwd launch" : "attn_fwd launch", tm, a);
 }
 
-template <int DH, bool kF16>
-int launch_bwd(const CUtensorMap &tm, const CUtensorMap &tmd, const AttnArgs &a, int B, cudaStream_t stream) {
+template <int DH, bool kF16, bool kX = false>
+int launch_bwd(const Maps<kX> &tm, const CUtensorMap &tmd, const AttnArgs &a, int B, cudaStream_t stream) {
     const dim3 grid((a.N + kRows - 1) / kRows, a.H, B);
-    if (int rc = launch(&attn_bwd_dq_kernel<DH, kF16>, smem_bytes<DH>(2), grid, stream, "attn_bwd_dq launch", tm, tmd, a)) return rc;
-    return launch(&attn_bwd_dkv_kernel<DH, kF16>, smem_bytes<DH>(2), grid, stream, "attn_bwd_dkv launch", tm, tmd, a);
+    if (int rc = launch(&attn_bwd_dq_kernel<DH, kF16, kX>, smem_bytes<DH>(2), grid, stream, kX ? "xattn_bwd_dq launch" : "attn_bwd_dq launch", tm, tmd, a))
+        return rc;
+    return launch(&attn_bwd_dkv_kernel<DH, kF16, kX>, smem_bytes<DH>(2), grid, stream, kX ? "xattn_bwd_dkv launch" : "attn_bwd_dkv launch", tm, tmd, a);
+}
+
+// The cross-attention entries' checks besides check_sizes: head dim 64 and 1 <= seg <= N.
+int check_xsizes(const char *what, int B, int N, int H, int dh, int seg, int dtype) {
+    if (int rc = check_sizes(what, B, N, H, dh, dtype)) return rc;
+    if (dh != 64) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "%s: head dim %d is not 64", what, dh);
+    if (seg < 1 || seg > N) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "%s: segment length %d is not in [1, N = %d]", what, seg, N);
+    return MIA_GEMM_OK;
 }
 
 AttnArgs make_args(int N, int H, int dh) {
@@ -482,8 +560,8 @@ int mia_attn_fwd(const void *qkv, void *o, float *lse, int B, int N, int H, int 
     if (((uintptr_t)qkv | (uintptr_t)o | (uintptr_t)lse) & 15) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "attn_fwd: qkv, o and lse must be 16-byte aligned");
     mia::DeviceInfo di;
     if (mia::device_info(mia::kErrGemm, di) != MIA_OK) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "attn_fwd: cannot query the device");
-    CUtensorMap tm;
-    if (int rc = make_map3(&tm, qkv, 3 * C, N, B, ld_qkv, dtype, what)) return rc;
+    Maps<false> tm;
+    if (int rc = make_map3(&tm.m[0], qkv, 3 * C, N, B, ld_qkv, dtype, what)) return rc;
     AttnArgs a = make_args(N, H, dh);
     a.o = o; a.ld_o = ld_o; a.lse_out = lse;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
@@ -509,8 +587,9 @@ int mia_attn_bwd(const void *qkv, const void *o, const void *dout, const float *
         return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "attn_bwd: qkv, o, dout, lse, delta and dqkv must be 16-byte aligned");
     mia::DeviceInfo di;
     if (mia::device_info(mia::kErrGemm, di) != MIA_OK) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "attn_bwd: cannot query the device");
-    CUtensorMap tm, tmd;
-    if (int rc = make_map3(&tm, qkv, 3 * C, N, B, ld_qkv, dtype, what)) return rc;
+    Maps<false> tm;
+    CUtensorMap tmd;
+    if (int rc = make_map3(&tm.m[0], qkv, 3 * C, N, B, ld_qkv, dtype, what)) return rc;
     if (int rc = make_map3(&tmd, dout, C, N, B, ld_do, dtype, what)) return rc;
     AttnArgs a = make_args(N, H, dh);
     a.o = const_cast<void *>(o); a.dout = dout; a.lse = lse; a.delta = delta; a.dqkv = dqkv;
@@ -522,6 +601,55 @@ int mia_attn_bwd(const void *qkv, const void *o, const void *dout, const float *
         case 64: return f16 ? launch_bwd<64, true>(tm, tmd, a, B, stream) : launch_bwd<64, false>(tm, tmd, a, B, stream);
         default: return f16 ? launch_bwd<80, true>(tm, tmd, a, B, stream) : launch_bwd<80, false>(tm, tmd, a, B, stream);
     }
+}
+
+int mia_xattn_fwd(const void *q, const void *kv, void *o, float *lse, int B, int N, int H, int dh, int seg, long long ld_q, long long ld_kv,
+                  long long ld_o, int dtype, void *cuda_stream) {
+    const char *what = "xattn_fwd";
+    if (!q || !kv || !o) return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "xattn_fwd: null pointer (q, kv and o are required)");
+    if (int rc = check_xsizes(what, B, N, H, dh, seg, dtype)) return rc;
+    const long long C = (long long)H * dh;
+    if (!pitch_ok(ld_q, C) || !pitch_ok(ld_kv, 2 * C) || !pitch_ok(ld_o, C))
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "xattn_fwd: row pitches must cover a row and be multiples of 8 elements "
+                         "(ld_q %lld, ld_o %lld >= C = %lld; ld_kv %lld >= 2C)", ld_q, ld_o, C, ld_kv);
+    if (((uintptr_t)q | (uintptr_t)kv | (uintptr_t)o | (uintptr_t)lse) & 15)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "xattn_fwd: q, kv, o and lse must be 16-byte aligned");
+    mia::DeviceInfo di;
+    if (mia::device_info(mia::kErrGemm, di) != MIA_OK) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "xattn_fwd: cannot query the device");
+    Maps<true> tm;
+    if (int rc = make_map3(&tm.m[0], q, C, N, B, ld_q, dtype, what)) return rc;
+    if (int rc = make_map3(&tm.m[1], kv, 2 * C, N, B, ld_kv, dtype, what)) return rc;
+    AttnArgs a = make_args(N, H, dh);
+    a.o = o; a.ld_o = ld_o; a.lse_out = lse; a.seg = seg;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    return dtype == MIA_GEMM_F16 ? launch_fwd<64, true, true>(tm, a, B, stream) : launch_fwd<64, false, true>(tm, a, B, stream);
+}
+
+int mia_xattn_bwd(const void *q, const void *kv, const void *o, const void *dout, const float *lse, float *delta, void *dq, void *dkv, int B, int N,
+                  int H, int dh, int seg, long long ld_q, long long ld_kv, long long ld_o, long long ld_do, long long ld_dq, long long ld_dkv, int dtype,
+                  void *cuda_stream) {
+    const char *what = "xattn_bwd";
+    if (!q || !kv || !o || !dout || !lse || !delta || !dq || !dkv)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "xattn_bwd: null pointer (q, kv, o, dout, lse, delta, dq and dkv are required)");
+    if (int rc = check_xsizes(what, B, N, H, dh, seg, dtype)) return rc;
+    const long long C = (long long)H * dh;
+    if (!pitch_ok(ld_q, C) || !pitch_ok(ld_kv, 2 * C) || !pitch_ok(ld_o, C) || !pitch_ok(ld_do, C) || !pitch_ok(ld_dq, C) || !pitch_ok(ld_dkv, 2 * C))
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "xattn_bwd: row pitches must cover a row and be multiples of 8 elements "
+                         "(ld_q %lld, ld_o %lld, ld_do %lld, ld_dq %lld >= C = %lld; ld_kv %lld, ld_dkv %lld >= 2C)", ld_q, ld_o, ld_do, ld_dq, C, ld_kv, ld_dkv);
+    if (((uintptr_t)q | (uintptr_t)kv | (uintptr_t)o | (uintptr_t)dout | (uintptr_t)lse | (uintptr_t)delta | (uintptr_t)dq | (uintptr_t)dkv) & 15)
+        return mia::fail(mia::kErrGemm, MIA_GEMM_EINVAL, "xattn_bwd: q, kv, o, dout, lse, delta, dq and dkv must be 16-byte aligned");
+    mia::DeviceInfo di;
+    if (mia::device_info(mia::kErrGemm, di) != MIA_OK) return mia::fail(mia::kErrGemm, MIA_GEMM_ECUDA, "xattn_bwd: cannot query the device");
+    Maps<true> tm;
+    CUtensorMap tmd;
+    if (int rc = make_map3(&tm.m[0], q, C, N, B, ld_q, dtype, what)) return rc;
+    if (int rc = make_map3(&tm.m[1], kv, 2 * C, N, B, ld_kv, dtype, what)) return rc;
+    if (int rc = make_map3(&tmd, dout, C, N, B, ld_do, dtype, what)) return rc;
+    AttnArgs a = make_args(N, H, dh);
+    a.o = const_cast<void *>(o); a.dout = dout; a.lse = lse; a.delta = delta; a.dqkv = dq; a.dkv = dkv; a.seg = seg;
+    a.ld_o = ld_o; a.ld_do = ld_do; a.ld_dqkv = ld_dq; a.ld_dkv = ld_dkv;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    return dtype == MIA_GEMM_F16 ? launch_bwd<64, true, true>(tm, tmd, a, B, stream) : launch_bwd<64, false, true>(tm, tmd, a, B, stream);
 }
 
 }  // extern "C"

@@ -74,6 +74,21 @@ def _mn_ok(t: torch.Tensor) -> bool:
     return t.dim() == 2 and t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0
 
 
+def rows_in(x: torch.Tensor, T: torch.dtype, K: int) -> torch.Tensor:
+    """x as a (M, K) operand in dtype T that the wgmma GEMM reads in place (copied only when its rows are not)."""
+    x2 = x.to(T).reshape(-1, K)
+    return x2 if _mn_ok(x2) else x2.contiguous()
+
+
+def linear_backward(dy2, x2, weight, bias, need_x, need_w, need_b, w_dtype, b_dtype, T):
+    """The gradients of y = x W^T + b from dy2 (M, N) and x2 (M, K), both in dtype T: dx = dy . W with W read MN-major,
+    dW = dy^T x in fp32 with both operands read in place, db = the fp32 column sum of dy; each None unless asked for."""
+    dx = gemm(dy2, weight.to(T).contiguous(), False, True) if need_x else None
+    dw = gemm(dy2, x2, True, True, torch.float32).to(w_dtype) if need_w else None
+    db = dy2.sum(0, dtype=torch.float32).to(b_dtype) if need_b and bias is not None else None
+    return dx, dw, db
+
+
 def transpose2d(t: torch.Tensor) -> torch.Tensor:
     """(R, C) -> contiguous (C, R)."""
     return t.t().contiguous()

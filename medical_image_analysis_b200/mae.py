@@ -101,9 +101,7 @@ class AttentionFn(torch.autograd.Function):
             raise RuntimeError(f"attention_fn: head dim C / num_heads = {C} / {num_heads} must be one of {ATTN_HEAD_DIMS}")
         if tuple(qkv_weight.shape) != (3 * C, C) or tuple(proj_weight.shape) != (C, C):
             raise RuntimeError(f"attention_fn: weights {tuple(qkv_weight.shape)} / {tuple(proj_weight.shape)} do not match C = {C}")
-        x2 = x.to(T).reshape(B * N, C)
-        if not _gemm._mn_ok(x2):
-            x2 = x2.contiguous()
+        x2 = _gemm.rows_in(x, T, C)
         ctx.sizes = (B, N, C, num_heads, T, checkpoint_lvl)
         qkv, o, lse = AttentionFn._attend(x2, qkv_weight, qkv_bias, ctx, train)
         y = _gemm.gemm_tn(o, proj_weight.to(T), proj_bias)
@@ -131,27 +129,15 @@ class AttentionFn(torch.autograd.Function):
         dev = x2.device
         need_x, need_wq, need_bq, need_wp, need_bp = ctx.needs_input_grad[:5]
         qkv, o, lse = keep if lvl == 0 else AttentionFn._attend(x2, wq, bq, ctx, True)
-        dy2 = dy.to(T).reshape(B * N, C)
-        if not _gemm._mn_ok(dy2):
-            dy2 = dy2.contiguous()
-        dx = dwq = dbq = dwp = dbp = None
-        if need_wp:                                                # dWp = dy^T o
-            dwp = _gemm.gemm(dy2, o, True, True, torch.float32).to(ctx.param_dtypes[2])
-        if need_bp and bp is not None:
-            dbp = dy2.sum(0, dtype=torch.float32).to(ctx.param_dtypes[3])
-        do = _gemm.gemm(dy2, wp.to(T).contiguous(), False, True)   # dO = dy . Wp (Wp read MN-major)
+        dy2 = _gemm.rows_in(dy, T, C)
+        do, dwp, dbp = _gemm.linear_backward(dy2, o, wp, bp, True, need_wp, need_bp, *ctx.param_dtypes[2:], T)   # dO = dy . Wp
         delta = torch.empty((B, H, N), dtype=torch.float32, device=dev)
         dqkv = torch.empty((B * N, 3 * C), dtype=T, device=dev)
         _lib.call("mia_attn_bwd", "attention_fn backward", dev, qkv.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr(), delta.data_ptr(),
                   dqkv.data_ptr(), B, N, H, C // H, qkv.stride(0), o.stride(0), do.stride(0), dqkv.stride(0), _lib.dtype_code(T))
         del qkv, o, lse, do, delta
-        if need_x:                                                 # dx = dqkv . Wq (Wq read MN-major)
-            dx = _gemm.gemm(dqkv, wq.to(T).contiguous(), False, True).view(B, N, C)
-        if need_wq:                                                # dWq = dqkv^T x
-            dwq = _gemm.gemm(dqkv, x2, True, True, torch.float32).to(ctx.param_dtypes[0])
-        if need_bq and bq is not None:
-            dbq = dqkv.sum(0, dtype=torch.float32).to(ctx.param_dtypes[1])
-        return dx, dwq, dbq, dwp, dbp, None, None, None
+        dx, dwq, dbq = _gemm.linear_backward(dqkv, x2, wq, bq, need_x, need_wq, need_bq, *ctx.param_dtypes[:2], T)
+        return None if dx is None else dx.view(B, N, C), dwq, dbq, dwp, dbp, None, None, None
 
 
 def attention_fn(x, qkv_weight, qkv_bias, proj_weight, proj_bias, num_heads, checkpoint_lvl=0):
