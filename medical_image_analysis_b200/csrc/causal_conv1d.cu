@@ -243,36 +243,20 @@ int conv_check(ConvArgs &a, const void *x, int batch, int dim, int L, int width,
     return MIA_OK;
 }
 
-template <typename T>
-void launch_conv_fwd(const ConvArgs &a, dim3 grid, int rpb, uint32_t magic, size_t smem, cudaStream_t st) {
-#define MIA_CONV_FWD(W)                                                                              \
-    do {                                                                                             \
-        if (a.silu) causal_conv1d_fwd_kernel<T, W, true><<<grid, kConvThreads, smem, st>>>(a, rpb, magic);  \
-        else causal_conv1d_fwd_kernel<T, W, false><<<grid, kConvThreads, smem, st>>>(a, rpb, magic);        \
-    } while (0)
-    switch (a.width) {
-        case 4: MIA_CONV_FWD(4); break;
-        case 3: MIA_CONV_FWD(3); break;
-        case 2: MIA_CONV_FWD(2); break;
-        default: MIA_CONV_FWD(1); break;
+// Calls f(std::integral_constant<int, W>{}, std::integral_constant<bool, S>{}) for the conv width W (1-4, anything else as 1:
+// callers validate it first) and the SiLU flag S, so that a launcher names each kernel once.
+template <typename F>
+void dispatch_conv(int width, int silu, F &&f) {
+    const auto with_act = [&](auto w) {
+        if (silu) f(w, std::true_type{});
+        else f(w, std::false_type{});
+    };
+    switch (width) {
+        case 4: with_act(std::integral_constant<int, 4>{}); break;
+        case 3: with_act(std::integral_constant<int, 3>{}); break;
+        case 2: with_act(std::integral_constant<int, 2>{}); break;
+        default: with_act(std::integral_constant<int, 1>{}); break;
     }
-#undef MIA_CONV_FWD
-}
-
-template <typename T>
-void launch_conv_bwd(const ConvArgs &a, uint32_t magic, cudaStream_t st) {
-#define MIA_CONV_BWD(W)                                                                              \
-    do {                                                                                             \
-        if (a.silu) causal_conv1d_bwd_kernel<T, W, true><<<a.dim, kConvThreads, 0, st>>>(a, magic);  \
-        else causal_conv1d_bwd_kernel<T, W, false><<<a.dim, kConvThreads, 0, st>>>(a, magic);        \
-    } while (0)
-    switch (a.width) {
-        case 4: MIA_CONV_BWD(4); break;
-        case 3: MIA_CONV_BWD(3); break;
-        case 2: MIA_CONV_BWD(2); break;
-        default: MIA_CONV_BWD(1); break;
-    }
-#undef MIA_CONV_BWD
 }
 
 // ------------------------------------------------------------------------------------------------ tile kernels
@@ -473,13 +457,46 @@ __global__ void conv_bwd_ex_finalize(const TileArgs a, const int kw) {
     else if (a.dbias) a.dbias[c] = s;
 }
 
+struct NoScale { __device__ __forceinline__ float operator()(float v) const { return v; } };
+
+// The SiLU gate's arithmetic on a staged tile, written once for the inner block's gate kernels and the multi-direction ones
+// (which scale by 1 / divisor): forward os = scale(os silu(zs)).
+template <typename Scale>
+__device__ __forceinline__ void gate_fwd_rows(float *os, const float *zs, Scale scale) {
+    constexpr int P = kTT + 1;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+    for (int rr = 0; rr < kRowsPerWarp; ++rr) {
+        const int r = warp + rr * kTileWarps;
+        for (int j = lane; j < kTT; j += 32) {
+            const float zv = zs[r * P + j];
+            os[r * P + j] = scale(os[r * P + j] * (zv * sigmoid_f(zv)));
+        }
+    }
+}
+
+// Backward, for g = scale(gs): gs = g silu(zs) (the gradient of the gated sum os), os = g os silu'(zs) (the gradient of zs).
+template <typename Scale>
+__device__ __forceinline__ void gate_bwd_rows(float *gs, float *os, const float *zs, Scale scale) {
+    constexpr int P = kTT + 1;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+    for (int rr = 0; rr < kRowsPerWarp; ++rr) {
+        const int r = warp + rr * kTileWarps;
+        for (int j = lane; j < kTT; j += 32) {
+            const float g = scale(gs[r * P + j]), zv = zs[r * P + j], s = sigmoid_f(zv);
+            gs[r * P + j] = g * (zv * s);
+            os[r * P + j] = g * os[r * P + j] * s * fmaf(zv, 1.f - s, 1.f);
+        }
+    }
+}
+
 // Gate forward: v = (in[0] + in[1] + ...) silu(z) -> every out[i].
 template <typename T>
 __global__ void __launch_bounds__(kTileThreads) gate_fwd_ex_kernel(const TileArgs a) {
     constexpr int P = kTT + 1;
     __shared__ float os[kTC * P], zs[kTC * P];
     const int c0 = blockIdx.x * kTC, t0 = blockIdx.y * kTT, b = blockIdx.z;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     tile_ld<T, false>(zs, P, a.z, b, c0, t0, kTT, a.dim, a.L);
     tile_ld<T, false>(os, P, a.in[0], b, c0, t0, kTT, a.dim, a.L);
     for (int i = 1; i < a.n_in; ++i) {
@@ -487,14 +504,7 @@ __global__ void __launch_bounds__(kTileThreads) gate_fwd_ex_kernel(const TileArg
         tile_ld<T, true>(os, P, a.in[i], b, c0, t0, kTT, a.dim, a.L);
     }
     __syncthreads();
-#pragma unroll
-    for (int rr = 0; rr < kRowsPerWarp; ++rr) {
-        const int r = warp + rr * kTileWarps;
-        for (int j = lane; j < kTT; j += 32) {
-            const float zv = zs[r * P + j];
-            os[r * P + j] *= zv * sigmoid_f(zv);
-        }
-    }
+    gate_fwd_rows(os, zs, NoScale{});
     __syncthreads();
     for (int i = 0; i < a.n_out; ++i) tile_st<T>(os, P, a.out[i], b, c0, t0, a.dim, a.L);
 }
@@ -507,7 +517,6 @@ __global__ void __launch_bounds__(kTileThreads) gate_bwd_ex_kernel(const TileArg
     extern __shared__ float gate_smem[];                        // 3 tiles: 50 KB, above the static 48 KB
     float *gs = gate_smem, *os = gs + kTC * P, *zs = os + kTC * P;
     const int c0 = blockIdx.x * kTC, t0 = blockIdx.y * kTT, b = blockIdx.z;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     tile_ld<T, false>(gs, P, a.in[0], b, c0, t0, kTT, a.dim, a.L);
     tile_ld<T, false>(zs, P, a.z, b, c0, t0, kTT, a.dim, a.L);
     tile_ld<T, false>(os, P, a.in[1], b, c0, t0, kTT, a.dim, a.L);
@@ -516,25 +525,18 @@ __global__ void __launch_bounds__(kTileThreads) gate_bwd_ex_kernel(const TileArg
         tile_ld<T, true>(os, P, a.in[i], b, c0, t0, kTT, a.dim, a.L);
     }
     __syncthreads();
-#pragma unroll
-    for (int rr = 0; rr < kRowsPerWarp; ++rr) {
-        const int r = warp + rr * kTileWarps;
-        for (int j = lane; j < kTT; j += 32) {
-            const float g = gs[r * P + j], zv = zs[r * P + j], s = sigmoid_f(zv);
-            gs[r * P + j] = g * (zv * s);
-            os[r * P + j] = g * os[r * P + j] * s * fmaf(zv, 1.f - s, 1.f);
-        }
-    }
+    gate_bwd_rows(gs, os, zs, NoScale{});
     __syncthreads();
     for (int i = 0; i < a.n_out; ++i) tile_st<TD>(gs, P, a.out[i], b, c0, t0, a.dim, a.L);
     tile_st<T>(os, P, a.dz, b, c0, t0, a.dim, a.L);
 }
 
-// Parts of the conv backward: ~8 CTAs per SM of a 132-SM H100 over all channel tiles.  A function of the sizes only, so the
-// order of the dweight / dbias sums (and therefore their bits) does not depend on the device.
-int conv_bwd_ex_parts(int batch, int dim, int L) {
+// Parts of the conv backward: ~8 CTAs per SM of a 132-SM H100 over all channel tiles of the n directions (n = 1 for the inner
+// block's kernel).  A function of the sizes only, so the order of the dweight / dbias sums (and therefore their bits) does not
+// depend on the device.
+int conv_bwd_parts(int n, int batch, int dim, int L) {
     const int ctiles = (dim + kTC - 1) / kTC, items = batch * ((L + kTT - 1) / kTT);
-    const int want = (8 * 132 + ctiles - 1) / ctiles;
+    const int want = (8 * 132 + ctiles * n - 1) / (ctiles * n);
     return want < items ? want : items;
 }
 
@@ -792,7 +794,6 @@ __global__ void __launch_bounds__(kTileThreads) gate_fwd_dirs_kernel(const DirAr
     constexpr int P = kTT + 1;
     __shared__ float os[kTC * P], zs[kTC * P];
     const int c0 = blockIdx.x * kTC, t0 = blockIdx.y * kTT, b = blockIdx.z;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     tile_ld<T, false>(zs, P, a.z, b, c0, t0, kTT, a.dim, a.L);
     for (int k = 0; k < a.o.n; ++k) {
         const auto pos = [&](int i) { return order_pos(a.o, k, i); };
@@ -804,14 +805,7 @@ __global__ void __launch_bounds__(kTileThreads) gate_fwd_dirs_kernel(const DirAr
         }
     }
     __syncthreads();
-#pragma unroll
-    for (int rr = 0; rr < kRowsPerWarp; ++rr) {
-        const int r = warp + rr * kTileWarps;
-        for (int j = lane; j < kTT; j += 32) {
-            const float zv = zs[r * P + j];
-            os[r * P + j] = os[r * P + j] * (zv * sigmoid_f(zv)) * a.scale;
-        }
-    }
+    gate_fwd_rows(os, zs, [&](float v) { return v * a.scale; });
     __syncthreads();
     tile_st<T>(os, P, a.y, b, c0, t0, a.dim, a.L);
 }
@@ -824,7 +818,6 @@ __global__ void __launch_bounds__(kTileThreads) gate_bwd_dirs_kernel(const DirAr
     extern __shared__ float gate_smem[];                        // 3 tiles: 50 KB, above the static 48 KB
     float *gs = gate_smem, *os = gs + kTC * P, *zs = os + kTC * P;
     const int c0 = blockIdx.x * kTC, t0 = blockIdx.y * kTT, b = blockIdx.z;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     tile_ld<T, false>(gs, P, a.y, b, c0, t0, kTT, a.dim, a.L);
     tile_ld<T, false>(zs, P, a.z, b, c0, t0, kTT, a.dim, a.L);
     for (int k = 0; k < a.o.n; ++k) {
@@ -837,36 +830,29 @@ __global__ void __launch_bounds__(kTileThreads) gate_bwd_dirs_kernel(const DirAr
         }
     }
     __syncthreads();
-#pragma unroll
-    for (int rr = 0; rr < kRowsPerWarp; ++rr) {
-        const int r = warp + rr * kTileWarps;
-        for (int j = lane; j < kTT; j += 32) {
-            const float g = gs[r * P + j] * a.scale, zv = zs[r * P + j], s = sigmoid_f(zv);
-            gs[r * P + j] = g * (zv * s);
-            os[r * P + j] = g * os[r * P + j] * s * fmaf(zv, 1.f - s, 1.f);
-        }
-    }
+    gate_bwd_rows(gs, os, zs, [&](float v) { return v * a.scale; });
     __syncthreads();
     for (int k = 0; k < a.o.n; ++k)
         tile_st_map<float>(gs, P, dense_op<float>(a.dense_out, a, k), b, c0, t0, a.dim, a.L, [&](int i) { return order_pos(a.o, k, i); });
     tile_st<T>(os, P, a.dz, b, c0, t0, a.dim, a.L);
 }
 
-// Parts of the multi-direction conv backward: conv_bwd_ex_parts's ~8 CTAs per SM shared by the directions.
-int conv_bwd_dirs_parts(int n, int batch, int dim, int L) {
-    const int ctiles = (dim + kTC - 1) / kTC, items = batch * ((L + kTT - 1) / kTT);
-    const int want = (8 * 132 + ctiles * n - 1) / (ctiles * n);
-    return want < items ? want : items;
-}
-
 bool op_ok(const mia_bdl *o) { return o && o->ptr; }
 Op op_of(const mia_bdl *o) { return op_ok(o) ? Op{o->ptr, o->batch_stride, o->d_stride, o->seq_stride} : Op{nullptr, 0, 0, 0}; }
 
-// Checks shared by the four entry points; fills a.in / a.out from the operand arrays.
+// Checks shared by the tile entry points: sizes (batch * z_per_batch CTAs fit the grid's z) and dtype.
+template <typename Args>
+int tile_check(const char *what, Args &a, int batch, int dim, int L, int dtype, int z_per_batch) {
+    if (batch <= 0 || dim <= 0 || L <= 0 || (long long)batch * z_per_batch > 65535) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: bad sizes", what);
+    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: bad dtype", what);
+    a.batch = batch; a.dim = dim; a.L = L;
+    return MIA_OK;
+}
+
+// Checks of the inner block's entry points; fills a.in / a.out from the operand arrays.
 int ex_check(const char *what, TileArgs &a, int batch, int dim, int L, int dtype, const mia_bdl *in, int n_in, int min_in,
              const mia_bdl *out, int n_out, int min_out) {
-    if (batch <= 0 || dim <= 0 || L <= 0 || batch > 65535) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: bad sizes", what);
-    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: bad dtype", what);
+    if (int rc = tile_check(what, a, batch, dim, L, dtype, 1)) return rc;
     if (n_in < min_in || n_in > kMaxOps || n_out < min_out || n_out > kMaxOps || (n_in && !in) || (n_out && !out)) {
         return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: %d inputs / %d outputs (at least %d / %d, at most %d each)", what, n_in, n_out,
                          min_in, min_out, kMaxOps);
@@ -879,20 +865,14 @@ int ex_check(const char *what, TileArgs &a, int batch, int dim, int L, int dtype
         if (!op_ok(out + i)) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: null output operand", what);
         a.out[i] = op_of(out + i);
     }
-    a.n_in = n_in; a.n_out = n_out; a.batch = batch; a.dim = dim; a.L = L;
+    a.n_in = n_in; a.n_out = n_out;
     return MIA_OK;
 }
 
-int ex_launched(const char *what) {
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? MIA_OK : mia::fail(mia::kErrConv, MIA_ECUDA, "%s launch: %s", what, cudaGetErrorString(e));
-}
-
-// Checks shared by the multi-direction entry points: sizes, dtype and the orders (a column order needs a square grid of
-// seqlen - 1 tokens).
+// Checks of the multi-direction entry points: tile_check and the orders (a column order needs a square grid of seqlen - 1
+// tokens).
 int dirs_check(const char *what, DirArgs &a, const int *orders, int n_dirs, int batch, int dim, int L, int dtype) {
-    if (batch <= 0 || dim <= 0 || L <= 0 || (long long)batch * kMaxDirs > 65535) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: bad sizes", what);
-    if (dtype != MIA_F32 && dtype != MIA_F16 && dtype != MIA_BF16) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: bad dtype", what);
+    if (int rc = tile_check(what, a, batch, dim, L, dtype, kMaxDirs)) return rc;
     if (!orders || n_dirs < 1 || n_dirs > kMaxDirs) return mia::fail(mia::kErrConv, MIA_EINVAL, "%s: 1-%d orders required, got %d", what, kMaxDirs, n_dirs);
     int side = 0;
     while ((side + 1) * (side + 1) <= L - 1) ++side;
@@ -905,7 +885,6 @@ int dirs_check(const char *what, DirArgs &a, const int *orders, int n_dirs, int 
         a.o.code[k] = c;
     }
     a.o.n = n_dirs; a.o.L = L; a.o.pos = L / 2; a.o.side = side;
-    a.batch = batch; a.dim = dim; a.L = L;
     return MIA_OK;
 }
 
@@ -939,7 +918,10 @@ int mia_causal_conv1d_fwd(const void *x, const float *weight, const float *bias,
     const size_t smem = (size_t)rpb * (width + 1) * sizeof(float);
     mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
-        launch_conv_fwd<T>(a, grid, rpb, mia::div_magic(qpr), smem, (cudaStream_t)cuda_stream);
+        dispatch_conv(width, silu, [&](auto w, auto act) {
+            causal_conv1d_fwd_kernel<T, decltype(w)::value, decltype(act)::value>
+                <<<grid, kConvThreads, smem, (cudaStream_t)cuda_stream>>>(a, rpb, mia::div_magic(qpr));
+        });
     });
     return mia::launched(mia::kErrConv, "causal_conv1d_fwd launch");
 }
@@ -964,7 +946,9 @@ int mia_causal_conv1d_bwd(const void *x, const float *weight, const float *bias,
     }
     mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
-        launch_conv_bwd<T>(a, mia::div_magic(qpr), (cudaStream_t)cuda_stream);
+        dispatch_conv(width, silu, [&](auto w, auto act) {
+            causal_conv1d_bwd_kernel<T, decltype(w)::value, decltype(act)::value><<<dim, kConvThreads, 0, (cudaStream_t)cuda_stream>>>(a, mia::div_magic(qpr));
+        });
     });
     return mia::launched(mia::kErrConv, "causal_conv1d_bwd launch");
 }
@@ -983,16 +967,16 @@ int mia_causal_conv1d_fwd_ex(const mia_bdl *x, const float *weight, const float 
     cudaStream_t st = (cudaStream_t)cuda_stream;
     mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
-#define MIA_EX_FWD(W) (silu ? conv_fwd_ex_kernel<T, W, true><<<grid, kTileThreads, 0, st>>>(a) : conv_fwd_ex_kernel<T, W, false><<<grid, kTileThreads, 0, st>>>(a))
-        switch (width) { case 4: MIA_EX_FWD(4); break; case 3: MIA_EX_FWD(3); break; case 2: MIA_EX_FWD(2); break; default: MIA_EX_FWD(1); }
-#undef MIA_EX_FWD
+        dispatch_conv(width, silu, [&](auto w, auto act) {
+            conv_fwd_ex_kernel<T, decltype(w)::value, decltype(act)::value><<<grid, kTileThreads, 0, st>>>(a);
+        });
     });
-    return ex_launched(what);
+    return mia::launched(mia::kErrConv, "causal_conv1d_fwd_ex launch");
 }
 
 size_t mia_causal_conv1d_bwd_ex_workspace(int batch, int dim, int seqlen, int width) {
     if (batch <= 0 || dim <= 0 || seqlen <= 0 || width < 1 || width > kMaxW) return 0;
-    return (size_t)conv_bwd_ex_parts(batch, dim, seqlen) * dim * (width + 1) * sizeof(float);
+    return (size_t)conv_bwd_parts(1, batch, dim, seqlen) * dim * (width + 1) * sizeof(float);
 }
 
 int mia_causal_conv1d_bwd_ex(const mia_bdl *x, const float *weight, const float *bias, const mia_bdl *dys, int n_dys, const mia_bdl *dx,
@@ -1008,18 +992,18 @@ int mia_causal_conv1d_bwd_ex(const mia_bdl *x, const float *weight, const float 
         return mia::fail(mia::kErrConv, MIA_EWORKSPACE, "%s: workspace missing or too small", what);
     }
     a.x = op_of(x); a.dx = op_of(dx); a.w = weight; a.bias = bias; a.dw = dweight; a.dbias = dbias; a.part = (float *)workspace;
-    a.n_tt = (seqlen + kTT - 1) / kTT; a.parts = conv_bwd_ex_parts(batch, dim, seqlen);
+    a.n_tt = (seqlen + kTT - 1) / kTT; a.parts = conv_bwd_parts(1, batch, dim, seqlen);
     const dim3 grid((dim + kTC - 1) / kTC, a.parts);
     cudaStream_t st = (cudaStream_t)cuda_stream;
     mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
-#define MIA_EX_BWD(W) (silu ? conv_bwd_ex_kernel<T, W, true><<<grid, kTileThreads, 0, st>>>(a) : conv_bwd_ex_kernel<T, W, false><<<grid, kTileThreads, 0, st>>>(a))
-        switch (width) { case 4: MIA_EX_BWD(4); break; case 3: MIA_EX_BWD(3); break; case 2: MIA_EX_BWD(2); break; default: MIA_EX_BWD(1); }
-#undef MIA_EX_BWD
+        dispatch_conv(width, silu, [&](auto w, auto act) {
+            conv_bwd_ex_kernel<T, decltype(w)::value, decltype(act)::value><<<grid, kTileThreads, 0, st>>>(a);
+        });
     });
-    if (int rc = ex_launched(what)) return rc;
+    if (int rc = mia::launched(mia::kErrConv, "causal_conv1d_bwd_ex launch")) return rc;
     conv_bwd_ex_finalize<<<(dim * (width + 1) + 255) / 256, 256, 0, st>>>(a, width);
-    return ex_launched("causal_conv1d_bwd_ex finalize");
+    return mia::launched(mia::kErrConv, "causal_conv1d_bwd_ex finalize launch");
 }
 
 int mia_silu_gate_fwd_ex(const mia_bdl *outs, int n_outs, const mia_bdl *z, const mia_bdl *out_zs, int n_out_zs, int batch, int dim, int seqlen,
@@ -1034,7 +1018,7 @@ int mia_silu_gate_fwd_ex(const mia_bdl *outs, int n_outs, const mia_bdl *z, cons
         using T = typename std::remove_pointer<decltype(tag)>::type;
         gate_fwd_ex_kernel<T><<<grid, kTileThreads, 0, (cudaStream_t)cuda_stream>>>(a);
     });
-    return ex_launched(what);
+    return mia::launched(mia::kErrConv, "silu_gate_fwd_ex launch");
 }
 
 int mia_silu_gate_bwd_ex(const mia_bdl *dy, const mia_bdl *outs, int n_outs, const mia_bdl *z, const mia_bdl *douts, int n_douts, const mia_bdl *dz,
@@ -1062,7 +1046,7 @@ int mia_silu_gate_bwd_ex(const mia_bdl *dy, const mia_bdl *outs, int n_outs, con
         return e;
     });
     if (int rc = mia::cuda_fail(mia::kErrConv, what, e)) return rc;
-    return ex_launched(what);
+    return mia::launched(mia::kErrConv, "silu_gate_bwd_ex launch");
 }
 
 // ---- ARM's multi-direction (bimamba v3) kernels (see "scan orders" above)
@@ -1083,16 +1067,16 @@ int mia_causal_conv1d_fwd_dirs(const mia_bdl *x, const int *orders, int n_dirs, 
     cudaStream_t st = (cudaStream_t)cuda_stream;
     mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
-#define MIA_DIRS_FWD(W) (silu ? conv_fwd_dirs_kernel<T, W, true><<<grid, kTileThreads, 0, st>>>(a) : conv_fwd_dirs_kernel<T, W, false><<<grid, kTileThreads, 0, st>>>(a))
-        switch (width) { case 4: MIA_DIRS_FWD(4); break; case 3: MIA_DIRS_FWD(3); break; case 2: MIA_DIRS_FWD(2); break; default: MIA_DIRS_FWD(1); }
-#undef MIA_DIRS_FWD
+        dispatch_conv(width, silu, [&](auto w, auto act) {
+            conv_fwd_dirs_kernel<T, decltype(w)::value, decltype(act)::value><<<grid, kTileThreads, 0, st>>>(a);
+        });
     });
-    return ex_launched(what);
+    return mia::launched(mia::kErrConv, "causal_conv1d_fwd_dirs launch");
 }
 
 size_t mia_causal_conv1d_bwd_dirs_workspace(int n_dirs, int batch, int dim, int seqlen, int width) {
     if (n_dirs < 1 || n_dirs > kMaxDirs || batch <= 0 || dim <= 0 || seqlen <= 0 || width < 1 || width > kMaxW) return 0;
-    return ((size_t)n_dirs * batch * dim * seqlen + (size_t)n_dirs * conv_bwd_dirs_parts(n_dirs, batch, dim, seqlen) * dim * (width + 1)) *
+    return ((size_t)n_dirs * batch * dim * seqlen + (size_t)n_dirs * conv_bwd_parts(n_dirs, batch, dim, seqlen) * dim * (width + 1)) *
            sizeof(float);
 }
 
@@ -1114,17 +1098,17 @@ int mia_causal_conv1d_bwd_dirs(const mia_bdl *x, const int *orders, int n_dirs, 
     }
     a.x = op_of(x); a.dx = op_of(dx); a.w = weight; a.bias = bias; a.dw = dweight; a.dbias = dbias; a.dense = du; a.has_tm = dy_tm != nullptr;
     a.xpart = (float *)workspace; a.part = a.xpart + (size_t)n_dirs * batch * dim * seqlen;
-    a.n_tt = (seqlen + kTT - 1) / kTT; a.parts = conv_bwd_dirs_parts(n_dirs, batch, dim, seqlen);
+    a.n_tt = (seqlen + kTT - 1) / kTT; a.parts = conv_bwd_parts(n_dirs, batch, dim, seqlen);
     const dim3 grid((dim + kTC - 1) / kTC, a.parts, n_dirs), fgrid((dim + kTC - 1) / kTC, a.n_tt, batch);
     cudaStream_t st = (cudaStream_t)cuda_stream;
     mia::dispatch_dtype(dtype, [&](auto *tag) {
         using T = typename std::remove_pointer<decltype(tag)>::type;
-#define MIA_DIRS_BWD(W) (silu ? conv_bwd_dirs_kernel<T, W, true><<<grid, kTileThreads, 0, st>>>(a) : conv_bwd_dirs_kernel<T, W, false><<<grid, kTileThreads, 0, st>>>(a))
-        switch (width) { case 4: MIA_DIRS_BWD(4); break; case 3: MIA_DIRS_BWD(3); break; case 2: MIA_DIRS_BWD(2); break; default: MIA_DIRS_BWD(1); }
-#undef MIA_DIRS_BWD
+        dispatch_conv(width, silu, [&](auto w, auto act) {
+            conv_bwd_dirs_kernel<T, decltype(w)::value, decltype(act)::value><<<grid, kTileThreads, 0, st>>>(a);
+        });
         if (cudaPeekAtLastError() == cudaSuccess) conv_bwd_dirs_finalize<T><<<fgrid, kTileThreads, 0, st>>>(a, width);
     });
-    return ex_launched(what);
+    return mia::launched(mia::kErrConv, "causal_conv1d_bwd_dirs launch");
 }
 
 int mia_silu_gate_fwd_dirs(const void *outs, const int *orders, int n_dirs, int divisor, const mia_bdl *z, const mia_bdl *y, int batch, int dim,
@@ -1139,7 +1123,7 @@ int mia_silu_gate_fwd_dirs(const void *outs, const int *orders, int n_dirs, int 
         using T = typename std::remove_pointer<decltype(tag)>::type;
         gate_fwd_dirs_kernel<T><<<grid, kTileThreads, 0, (cudaStream_t)cuda_stream>>>(a);
     });
-    return ex_launched(what);
+    return mia::launched(mia::kErrConv, "silu_gate_fwd_dirs launch");
 }
 
 int mia_silu_gate_bwd_dirs(const mia_bdl *dy, const void *outs, const int *orders, int n_dirs, int divisor, const mia_bdl *z, float *douts,
@@ -1160,7 +1144,7 @@ int mia_silu_gate_bwd_dirs(const mia_bdl *dy, const void *outs, const int *order
         return e;
     });
     if (int rc = mia::cuda_fail(mia::kErrConv, what, e)) return rc;
-    return ex_launched(what);
+    return mia::launched(mia::kErrConv, "silu_gate_bwd_dirs launch");
 }
 
 }  // extern "C"
