@@ -410,7 +410,9 @@ __global__ void __launch_bounds__(32, 8) ss_bwd_cw_kernel(const __grid_constant_
 template <typename T, int kG>
 cudaError_t launch_bwd_cw_g(const CUtensorMap *tm, const CwBwdArgs &a, int grid, bool dout_f32, cudaStream_t stream) {
     void (*kernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CwBwdArgs);
-    if (a.softplus) kernel = dout_f32 ? &ss_bwd_cw_kernel<T, true, true, kG> : &ss_bwd_cw_kernel<T, true, false, kG>;
+    if constexpr (sizeof(T) == 4)        // fp32 inputs: dout is T, dout_f32 is never set (scan_api.cu)
+        kernel = a.softplus ? &ss_bwd_cw_kernel<T, true, false, kG> : &ss_bwd_cw_kernel<T, false, false, kG>;
+    else if (a.softplus) kernel = dout_f32 ? &ss_bwd_cw_kernel<T, true, true, kG> : &ss_bwd_cw_kernel<T, true, false, kG>;
     else kernel = dout_f32 ? &ss_bwd_cw_kernel<T, false, true, kG> : &ss_bwd_cw_kernel<T, false, false, kG>;
     return launch_smem(kernel, grid, 32, a.smem_bytes, stream, tm[0], tm[1], tm[2], tm[3], tm[4], a);
 }

@@ -233,13 +233,15 @@ cudaError_t launch_bwd_any(const ScanArgs &a, int grid, cudaStream_t stream) {
     const bool fast = a.LPR == 32 && a.delta_ratio == 1 && (a.N > 1 || !a.has_z);
     if (!fast) return launch_bwd<T>(a, grid, stream);
     void (*kernel)(const ScanArgs);
-    const bool of32 = a.out_f32 || sizeof(T) == 4;
-    if (a.N == 1) {
-        if (a.softplus) kernel = of32 ? &ss_bwd_fast_kernel<T, true, true> : &ss_bwd_fast_kernel<T, true, false>;
-        else kernel = of32 ? &ss_bwd_fast_kernel<T, false, true> : &ss_bwd_fast_kernel<T, false, false>;
+    if constexpr (sizeof(T) == 4) {      // fp32 inputs read fp32 douts: kOutF32 is always set
+        if (a.N == 1) kernel = a.softplus ? &ss_bwd_fast_kernel<T, true, true> : &ss_bwd_fast_kernel<T, false, true>;
+        else kernel = a.softplus ? &ss_bwd_fastn_kernel<T, true, true> : &ss_bwd_fastn_kernel<T, false, true>;
+    } else if (a.N == 1) {
+        if (a.softplus) kernel = a.out_f32 ? &ss_bwd_fast_kernel<T, true, true> : &ss_bwd_fast_kernel<T, true, false>;
+        else kernel = a.out_f32 ? &ss_bwd_fast_kernel<T, false, true> : &ss_bwd_fast_kernel<T, false, false>;
     } else {
-        if (a.softplus) kernel = of32 ? &ss_bwd_fastn_kernel<T, true, true> : &ss_bwd_fastn_kernel<T, true, false>;
-        else kernel = of32 ? &ss_bwd_fastn_kernel<T, false, true> : &ss_bwd_fastn_kernel<T, false, false>;
+        if (a.softplus) kernel = a.out_f32 ? &ss_bwd_fastn_kernel<T, true, true> : &ss_bwd_fastn_kernel<T, true, false>;
+        else kernel = a.out_f32 ? &ss_bwd_fastn_kernel<T, false, true> : &ss_bwd_fastn_kernel<T, false, false>;
     }
     return launch_smem(kernel, grid, kThreads, a.smem_bytes, stream, a);
 }
@@ -252,9 +254,10 @@ cudaError_t launch_bwd_det(const ScanArgs &a, int grid, cudaStream_t stream) {
     const bool fast = a.LPR == 32 && a.delta_ratio == 1;
     if (!fast) return launch_bwd<T, true>(a, grid, stream);
     void (*kernel)(const ScanArgs);
-    const bool of32 = a.out_f32 || sizeof(T) == 4;
-    if (a.softplus) kernel = of32 ? &ss_bwd_fastn_kernel<T, true, true, true> : &ss_bwd_fastn_kernel<T, true, false, true>;
-    else kernel = of32 ? &ss_bwd_fastn_kernel<T, false, true, true> : &ss_bwd_fastn_kernel<T, false, false, true>;
+    if constexpr (sizeof(T) == 4)        // fp32 inputs read fp32 douts: kOutF32 is always set
+        kernel = a.softplus ? &ss_bwd_fastn_kernel<T, true, true, true> : &ss_bwd_fastn_kernel<T, false, true, true>;
+    else if (a.softplus) kernel = a.out_f32 ? &ss_bwd_fastn_kernel<T, true, true, true> : &ss_bwd_fastn_kernel<T, true, false, true>;
+    else kernel = a.out_f32 ? &ss_bwd_fastn_kernel<T, false, true, true> : &ss_bwd_fastn_kernel<T, false, false, true>;
     return launch_smem(kernel, grid, kThreads, a.smem_bytes, stream, a);
 }
 

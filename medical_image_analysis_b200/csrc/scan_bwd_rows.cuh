@@ -367,7 +367,9 @@ __global__ void __launch_bounds__(64, 5) ss_bwd_rows_kernel(const __grid_constan
 template <typename T>
 cudaError_t launch_bwd_rows(const RowsBwdArgs &a, int grid, bool dout_f32, cudaStream_t stream) {
     void (*kernel)(const RowsBwdArgs);
-    if (a.softplus) kernel = dout_f32 ? &ss_bwd_rows_kernel<T, true, true> : &ss_bwd_rows_kernel<T, true, false>;
+    if constexpr (sizeof(T) == 4)        // fp32 inputs: dout is T, dout_f32 is never set (scan_api.cu)
+        kernel = a.softplus ? &ss_bwd_rows_kernel<T, true, false> : &ss_bwd_rows_kernel<T, false, false>;
+    else if (a.softplus) kernel = dout_f32 ? &ss_bwd_rows_kernel<T, true, true> : &ss_bwd_rows_kernel<T, true, false>;
     else kernel = dout_f32 ? &ss_bwd_rows_kernel<T, false, true> : &ss_bwd_rows_kernel<T, false, false>;
     return launch_smem(kernel, grid, 64, a.smem_bytes, stream, a);
 }

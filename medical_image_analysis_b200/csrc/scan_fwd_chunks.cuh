@@ -156,7 +156,9 @@ template <typename T>
 cudaError_t launch_fwd_chunks(const ChunkArgs &a, int grid, bool out_f32, cudaStream_t stream) {
     void (*ka)(const ChunkArgs) = a.softplus ? &ss_fwd_chunk_kernel<T, true, false, true> : &ss_fwd_chunk_kernel<T, false, false, true>;
     void (*kc)(const ChunkArgs);
-    if (a.softplus) kc = out_f32 ? &ss_fwd_chunk_kernel<T, true, true, false> : &ss_fwd_chunk_kernel<T, true, false, false>;
+    if constexpr (sizeof(T) == 4)        // fp32 inputs: out is T, out_f32 is never set (scan_api.cu)
+        kc = a.softplus ? &ss_fwd_chunk_kernel<T, true, false, false> : &ss_fwd_chunk_kernel<T, false, false, false>;
+    else if (a.softplus) kc = out_f32 ? &ss_fwd_chunk_kernel<T, true, true, false> : &ss_fwd_chunk_kernel<T, true, false, false>;
     else kc = out_f32 ? &ss_fwd_chunk_kernel<T, false, true, false> : &ss_fwd_chunk_kernel<T, false, false, false>;
     const cudaError_t e = cudaFuncSetAttribute(ka, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smem_bytes);
     if (e != cudaSuccess) return e;

@@ -314,7 +314,9 @@ __global__ void __launch_bounds__(32, 16) ss_fwd_cw_kernel(const __grid_constant
 template <typename T, int kG>
 cudaError_t launch_fwd_cw_g(const CUtensorMap *tm, const CwFwdArgs &a, int grid, bool out_f32, cudaStream_t stream) {
     void (*kernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CwFwdArgs);
-    if (a.softplus) kernel = out_f32 ? &ss_fwd_cw_kernel<T, true, true, kG> : &ss_fwd_cw_kernel<T, true, false, kG>;
+    if constexpr (sizeof(T) == 4)        // fp32 inputs: out is T, out_f32 is never set (scan_api.cu)
+        kernel = a.softplus ? &ss_fwd_cw_kernel<T, true, false, kG> : &ss_fwd_cw_kernel<T, false, false, kG>;
+    else if (a.softplus) kernel = out_f32 ? &ss_fwd_cw_kernel<T, true, true, kG> : &ss_fwd_cw_kernel<T, true, false, kG>;
     else kernel = out_f32 ? &ss_fwd_cw_kernel<T, false, true, kG> : &ss_fwd_cw_kernel<T, false, false, kG>;
     return launch_smem(kernel, grid, 32, a.smem_bytes, stream, tm[0], tm[1], tm[2], a);
 }

@@ -156,9 +156,10 @@ cudaError_t launch_fwd_any(const ScanArgs &a, int grid, cudaStream_t stream) {
     const bool fast = a.N == 1 && a.LPR == 32 && !a.has_z && a.delta_ratio == 1;
     if (!fast) return launch_fwd<T>(a, grid, stream);
     void (*kernel)(const ScanArgs);
-    const bool of32 = a.out_f32 || sizeof(T) == 4;
-    if (a.softplus) kernel = of32 ? &ss_fwd_fast_kernel<T, true, true> : &ss_fwd_fast_kernel<T, true, false>;
-    else kernel = of32 ? &ss_fwd_fast_kernel<T, false, true> : &ss_fwd_fast_kernel<T, false, false>;
+    if constexpr (sizeof(T) == 4)        // fp32 inputs store fp32 outputs: kOutF32 is always set
+        kernel = a.softplus ? &ss_fwd_fast_kernel<T, true, true> : &ss_fwd_fast_kernel<T, false, true>;
+    else if (a.softplus) kernel = a.out_f32 ? &ss_fwd_fast_kernel<T, true, true> : &ss_fwd_fast_kernel<T, true, false>;
+    else kernel = a.out_f32 ? &ss_fwd_fast_kernel<T, false, true> : &ss_fwd_fast_kernel<T, false, false>;
     return launch_smem(kernel, grid, kThreadsFwd, a.smem_bytes, stream, a);
 }
 

@@ -260,8 +260,10 @@ __global__ void __launch_bounds__(32 * kRowsNWarps) ss_fwd_rowsn_kernel(const __
 
 template <typename T, int kN, bool kHasZ>
 void (*pick_fwd_rowsn(bool softplus, bool out_f32))(const RowsNArgs) {
-    if (softplus) return out_f32 ? &ss_fwd_rowsn_kernel<T, true, true, kN, kHasZ> : &ss_fwd_rowsn_kernel<T, true, false, kN, kHasZ>;
-    return out_f32 ? &ss_fwd_rowsn_kernel<T, false, true, kN, kHasZ> : &ss_fwd_rowsn_kernel<T, false, false, kN, kHasZ>;
+    if constexpr (sizeof(T) == 4)        // fp32 inputs: out is T, out_f32 is never set (scan_api.cu)
+        return softplus ? &ss_fwd_rowsn_kernel<T, true, false, kN, kHasZ> : &ss_fwd_rowsn_kernel<T, false, false, kN, kHasZ>;
+    else if (softplus) return out_f32 ? &ss_fwd_rowsn_kernel<T, true, true, kN, kHasZ> : &ss_fwd_rowsn_kernel<T, true, false, kN, kHasZ>;
+    else return out_f32 ? &ss_fwd_rowsn_kernel<T, false, true, kN, kHasZ> : &ss_fwd_rowsn_kernel<T, false, false, kN, kHasZ>;
 }
 
 template <typename T>

@@ -178,7 +178,9 @@ __global__ void __launch_bounds__(32, 16) ss_fwd_stream_kernel(const __grid_cons
 template <typename T>
 cudaError_t launch_fwd_stream(const StreamArgs &a, int grid, bool out_f32, cudaStream_t stream) {
     void (*kernel)(const StreamArgs);
-    if (a.softplus) kernel = out_f32 ? &ss_fwd_stream_kernel<T, true, true> : &ss_fwd_stream_kernel<T, true, false>;
+    if constexpr (sizeof(T) == 4)        // fp32 inputs: out is T, out_f32 is never set (scan_api.cu)
+        kernel = a.softplus ? &ss_fwd_stream_kernel<T, true, false> : &ss_fwd_stream_kernel<T, false, false>;
+    else if (a.softplus) kernel = out_f32 ? &ss_fwd_stream_kernel<T, true, true> : &ss_fwd_stream_kernel<T, true, false>;
     else kernel = out_f32 ? &ss_fwd_stream_kernel<T, false, true> : &ss_fwd_stream_kernel<T, false, false>;
     return launch_smem(kernel, grid, 32, a.smem_bytes, stream, a);
 }
