@@ -10,6 +10,7 @@ import os
 import re
 import subprocess
 import sys
+import time
 
 import torch
 
@@ -43,10 +44,14 @@ def launched(fn, pattern):
     return res, [e.name for e in prof.events() if rx.search(e.name)]
 
 
-def retry(run, complete, tries=3):
-    """Now and then a short profiler session loses kernel records: ``run()`` is taken again, up to ``tries`` times in all,
-    until ``complete(result)`` holds.  The last result is returned either way, so a wrong launch still fails the caller."""
-    for _ in range(tries):
+def retry(run, complete, tries=6, pause=0.25):
+    """Now and then a short profiler session loses kernel records, sometimes several sessions in a row: ``run()`` is taken
+    again, up to ``tries`` times in all, until ``complete(result)`` holds, waiting ``pause`` seconds times the number of
+    failed tries before each new one so that a burst of lost records can pass.  A complete first capture costs nothing
+    extra.  The last result is returned either way, so a wrong launch still fails the caller."""
+    for i in range(tries):
+        if i:
+            time.sleep(pause * i)
         res = run()
         if complete(res):
             break

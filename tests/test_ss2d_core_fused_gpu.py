@@ -28,13 +28,14 @@ def _module(ft, d_inner, N, seed=0):
 
 
 def _run(m, x, mode, composed, seed=9, **kw):
-    """-> (output, {name: grad}) of one forward + backward; mode fp32 / bf16 (module and input in bf16) / autocast."""
+    """-> (output, {name: grad}) of one forward + backward; mode fp32 / bf16 (module and input in bf16) / autocast (bf16) /
+    autocast_fp16."""
     x = x.detach().clone().requires_grad_()
     for p in m.parameters():
         p.grad = None
     fwd = m._forward_composed if composed else m.forward
-    if mode == "autocast":
-        with torch.autocast("cuda", dtype=torch.bfloat16):
+    if mode.startswith("autocast"):
+        with torch.autocast("cuda", dtype=torch.float16 if mode == "autocast_fp16" else torch.bfloat16):
             out = fwd(x)
     else:
         out = fwd(x)
@@ -185,11 +186,11 @@ def test_epilogue_matches_statement(shape, dt, gate):
 FT_CASES = [("v3noz", 1, 16, 6, 5), ("v3", 16, 32, 7, 9), ("v2", 4, 32, 14, 14), ("v4", 1, 64, 14, 14), ("v4noz", 4, 32, 7, 9),
             ("v3nozact", 1, 32, 6, 5), ("v2no32", 16, 32, 14, 14), ("v3noz", 1, 768, 14, 14), ("v3", 1, 192, 80, 80),
             ("v3noz", 1, 2048, 6, 5)]
-TOL = {"fp32": (2e-3, 6e-2), "bf16": (2e-2, 0.5), "autocast": (2e-2, 0.5)}
+TOL = {"fp32": (2e-3, 6e-2), "bf16": (2e-2, 0.5), "autocast": (2e-2, 0.5), "autocast_fp16": (2e-2, 0.5)}
 
 
 @gpu
-@pytest.mark.parametrize("mode", ["fp32", "bf16", "autocast"])
+@pytest.mark.parametrize("mode", ["fp32", "bf16", "autocast", "autocast_fp16"])
 @pytest.mark.parametrize("case", FT_CASES, ids=[f"{c[0]}_N{c[1]}_D{c[2]}_{c[3]}x{c[4]}" for c in FT_CASES])
 def test_fused_matches_composition(case, mode):
     ft, N, D, H, W = case
@@ -448,6 +449,38 @@ def test_kernel_path():
     assert not fwd["full_size_ops"], fwd["full_size_ops"]
     # the one full-size copy left: torch's in-place baddbmm_ (dx += W_x^T dZ on the merge output) stages its result once
     assert len(bwd["full_size_ops"]) <= 1 and all("aten::baddbmm_" in op for op in bwd["full_size_ops"]), bwd["full_size_ops"]
+
+
+def kernel_path_fp16():
+    """Run in a child interpreter: the epilogue and CrossScan1b1 kernels of one VSSM forward + backward under fp16 autocast."""
+    from medical_image_analysis_b200.vmamba import VSSM
+    torch.manual_seed(0)
+    model = VSSM(depths=[1], dims=[32], num_classes=10, drop_path_rate=0.0, forward_type="v3").cuda()
+    x = torch.randn(2, 3, 32, 32, device="cuda")
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        with torch.autocast("cuda", dtype=torch.float16):
+            out = model(x)
+        out.float().sum().backward()
+        torch.cuda.synchronize()
+    rx = re.compile(r"\b(merge_norm_\w+?|cross_1b1_(?:direct_)?kernel)(?=[<(])")
+    names = set()
+    for e in prof.events():
+        m = rx.search(e.name)
+        if m:
+            rest = e.name[m.end():]
+            names.add(m.group(1) + (f"<{', '.join(kernel_trace.targs(e.name, m.group(1) + '<'))}>" if rest.startswith("<") else ""))
+    return sorted(names)
+
+
+@gpu
+def test_kernel_path_fp16_autocast():
+    """Under fp16 autocast the activations reach the op as fp16: the v3 core's fp32 scan output is merged into an fp16 output
+    (merge_norm_fwd_kernel<float, __half>), the backward runs in fp16, and CrossScan1b1 moves fp16 planes."""
+    names = kernel_trace.in_child("tests.test_ss2d_core_fused_gpu:kernel_path_fp16")
+    assert "merge_norm_fwd_kernel<float, __half>" in names, names
+    assert {"merge_norm_bwd_kernel<__half>", "merge_norm_bwd_finalize"} <= set(names), names
+    assert any(n.startswith("cross_1b1_kernel<__half, ") for n in names), names
 
 
 # ---------------------------------------------------------------------------------------------------------- determinism
